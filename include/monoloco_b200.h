@@ -227,8 +227,9 @@ int mlb_laplace_std(const float* d_bi, int n_pass, int n_rows, int n_samples, ui
 enum { MLB_TASK_D = 0, MLB_TASK_X = 1, MLB_TASK_Y = 2, MLB_TASK_H = 3, MLB_TASK_W = 4, MLB_TASK_L = 5,
        MLB_TASK_ORI = 6, MLB_TASK_AUX = 7 };  /* trainer.py:40, losses.py:76-101 */
 
-typedef struct mlb_train_block {   /* one L-wide Linear (+BatchNorm1d+ReLU+Dropout) in forward order           */
-    int32_t K;                     /* in_features                                                              */
+typedef struct mlb_train_block {   /* one L-wide Linear (+BatchNorm1d+ReLU+Dropout) in forward order; every    */
+                                   /* shape is the caller's real one (L = linear_size, padding is internal)    */
+    int32_t K;                     /* in_features: input_size for block 0, linear_size for the others          */
     int32_t has_bn;                /* 0 only for LocoModel.w2 (architectures.py:59)                            */
     int32_t res_src;               /* index of the block whose output is added to this one's (x + y), or -1   */
     int32_t reserved;
@@ -252,7 +253,7 @@ typedef struct mlb_train_args {
     float p_dropout, bn_eps, bn_momentum;
     int32_t flags;                 /* reserved, must be 0                                                       */
     uint64_t drop_seed;            /* counter-RNG seed (must be the same in forward and backward)               */
-    const uint8_t* drop_mask;      /* optional explicit keep masks [n_bn_blocks][B][L] (parity tests)           */
+    const uint8_t* drop_mask;      /* optional explicit keep masks [n_bn_blocks][B][L], L = linear_size         */
     const float* x;                /* [B, input_size] pre-processed inputs                                      */
     float* out;                    /* [B, output_size]                                                          */
     const float* g_out;            /* backward only: dL/d(out) [B, output_size]                                 */
@@ -269,7 +270,11 @@ typedef struct mlb_train_args {
 } mlb_train_args;
 
 typedef struct mlb_train* mlb_train_handle;
-/* workspace for up to max_rows detections: saved activations, pre-BN outputs, gradients, transposed weights. */
+/* workspace for up to max_rows detections: saved activations, pre-BN outputs, gradients, transposed weights.
+ * linear_size: any width in [1, 2048] (larger ones fail here).  The step runs at the forward's padded width (next
+ * multiple of 128 up to 1024, of 256 up to 2048); when that differs from linear_size the workspace also holds
+ * zero-padded copies of the parameters, gradients and keep masks, written and read back inside the same launch, and
+ * every tensor in mlb_train_args / mlb_train_block keeps the caller's real shape. */
 int mlb_train_create(int device, int max_rows, int input_size, int linear_size, int n_blocks, mlb_train_handle* out);
 void mlb_train_destroy(mlb_train_handle h);
 int mlb_train_forward(mlb_train_handle h, const mlb_train_args* a, const mlb_train_block* blocks, void* stream);

@@ -238,7 +238,7 @@ def train_step(model, x, labels, tasks, lambdas=None, log_sigmas=None, drop_mask
 def phase_times(model):
     """[(phase type name, block, ms)] of the most recent train launch of `model` (profiling aid)."""
     ws = _WS.get(model)
-    names = ['PACK', 'FWD', 'FWD_FINAL', 'BWD_INIT', 'BWD_HEAD', 'BWD', 'DW']
+    names = ['PACK', 'FWD', 'FWD_FINAL', 'BWD_INIT', 'BWD_HEAD', 'BWD', 'DW', 'PAD', 'UNPAD']
     ns = (C.c_double * 64)()
     ty = (C.c_int * 64)()
     bk = (C.c_int * 64)()

@@ -1,4 +1,7 @@
-"""Time the fused train step (single cooperative launch) vs torch-eager CUDA autograd of the same step on cuda:0."""
+"""Time the fused train step (single cooperative launch) vs torch-eager CUDA autograd of the same step on cuda:0.
+
+    python tools/bench_train.py [B ...] [--width L] [--stages S]     (defaults: B = 4096 512, L = 1024, S = 3)"""
+import argparse
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -23,10 +26,27 @@ def timeit(fn, n=10, warm=3):
     return e0.elapsed_time(e1) / n
 
 
-for B in [int(v) for v in (sys.argv[1:] or ['4096', '512'])]:
-    sd = synthetic.make_state_dict('loco', 34, 9, 1024, 3, 7)
+ap = argparse.ArgumentParser()
+ap.add_argument('batch', type=int, nargs='*', default=[4096, 512])
+ap.add_argument('--width', type=int, default=1024, help='hidden width (linear_size), 1..2048')
+ap.add_argument('--stages', type=int, default=3)
+args = ap.parse_args()
+Lw, st = args.width, args.stages
+def _power_limit():
+    import subprocess   # read-only query of the card the numbers belong to
+    try:
+        r = subprocess.run(['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader', '-i', '0'],
+                           capture_output=True, text=True, timeout=20)
+        return r.stdout.strip() or 'unknown'
+    except Exception:
+        return 'unknown'
+
+
+print('%s, power limit %s, width %d, %d stages' % (torch.cuda.get_device_name(0), _power_limit(), Lw, st))
+for B in args.batch:
+    sd = synthetic.make_state_dict('loco', 34, 9, Lw, st, 7)
     PD = float(os.environ.get('MLB_BENCH_PDROP', '0.2'))
-    m = LocoModel(34, 9, 1024, p_dropout=PD, num_stage=3)
+    m = LocoModel(34, 9, Lw, p_dropout=PD, num_stage=st)
     m.load_state_dict({k: torch.from_numpy(np.array(v)) for k, v in sd.items()})
     m.cuda().train()
     x = torch.from_numpy(synthetic.make_inputs(B, 34, seed=3)).cuda()
@@ -58,6 +78,6 @@ for B in [int(v) for v in (sys.argv[1:] or ['4096', '512'])]:
         loss, _ = T.multi_task_loss(out, y, tasks)
         loss.backward()
     t_eager = timeit(eager)
-    fl = 3 * 16865280 * B
-    print("train step B=%5d: fused 1-launch %.3f ms (%.1f TFLOP/s) | drop-in autograd (2 launches) %.3f ms | torch-eager CUDA %.3f ms | x%.2f"
-          % (B, t_fused, fl / t_fused / 1e9, t_dropin, t_eager, t_eager / t_fused))
+    fl = 3 * 2 * (34 * Lw + (2 * st + 2) * Lw * Lw + 9 * Lw) * B   # forward + 2x backward multiply-adds of the Linears
+    print("train step L=%d B=%5d: fused 1-launch %.3f ms (%.1f TFLOP/s) | drop-in autograd (2 launches) %.3f ms | torch-eager CUDA %.3f ms | x%.2f"
+          % (Lw, B, t_fused, fl / t_fused / 1e9, t_dropin, t_eager, t_eager / t_fused))
