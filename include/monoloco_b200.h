@@ -90,11 +90,13 @@ int mlb_last_kernel(mlb_handle h);
  * one wave of FFMA row tiles, [3] one wave of tensor-core tiles -- mlb_forward picks the kernel family with them (no constants
  * from another box).  Returns 1 if measured, 0 if the defaults are in use (MLB_NO_CALIBRATE). */
 int mlb_kernel_times(mlb_handle h, double out_ms[4]);
-/* co-resident clusters of the tensor-core kernel on this device (= its persistent grid size), 0 if unavailable */
+/* co-resident CTA groups of the tensor-core kernel on this device (= its persistent grid size: floor(co-resident CTAs /
+ * (linear_size / 256)), capped by MLB_TC_CLUSTERS), 0 if unavailable.  The name predates the groups: they were thread-block
+ * clusters. */
 int mlb_tc_resident_clusters(mlb_handle h);
 /* device error word of this handle (mapped host memory; read it after a stream synchronisation): 0 = none,
- * 1 = a TMA/mbarrier wait timed out, 3 = grid-barrier time-out (whole-grid kernel), 4 = fused all-gather: a peer
- * rank did not signal its epoch within 20 s. */
+ * 1 = a TMA/mbarrier wait timed out, 3 = grid-barrier time-out (whole-grid kernel; the tensor-core kernel's CTA-group
+ * barrier after 20 s), 4 = fused all-gather: a peer rank did not signal its epoch within 20 s. */
 int mlb_device_error(mlb_handle h);
 
 /* ---- inference ---- */

@@ -533,10 +533,10 @@ bool mlb_tc_supported(int L);
 mlb_tc_state* mlb_tc_prepare(const float* blob_dev, const mlb_op* ops, int n_ops, int L, cudaStream_t st, cudaError_t* err);
 cudaError_t mlb_tc_repack(mlb_tc_state* t, const float* blob_dev, const mlb_op* ops, int n_ops, int L, cudaStream_t st);
 void mlb_tc_free(mlb_tc_state* t);
-int mlb_tc_clusters(const mlb_tc_state* t, int n_rows);
+int mlb_tc_groups(const mlb_tc_state* t, int n_rows);
 cudaError_t mlb_tc_launch(const mlb_tc_state* t, const FwdParams& p, cudaStream_t st);
 cudaError_t mlb_tc_set_marks(unsigned long long* ptr);
-int mlb_tc_max_clusters(const mlb_tc_state* t);
+int mlb_tc_max_groups(const mlb_tc_state* t);
 int mlb_tc_tile_rows();
 // forward_wide.cu
 size_t mlb_wide_slab_floats(const mlb_op* ops, int n_ops, int L, long long* slab_off);
@@ -571,7 +571,7 @@ struct mlb_model {
     bool wide2_disabled;
     float* res_scratch;
     size_t res_floats;
-    mlb_tc_state* tc;              // tensor-core kernel state (weight planes, cluster workspace), or null
+    mlb_tc_state* tc;              // tensor-core kernel state (weight planes, group workspace), or null
     int last_kernel;               // MLB_KERNEL_* of the most recent mlb_forward launch
     // per-wave times measured on this device at mlb_create (ms): FFMA cluster wave, row-tile wave = a + b * TM, tensor-core wave
     double t_cluster_wave, t_tile_a, t_tile_b, t_tc_wave;
@@ -630,7 +630,7 @@ extern "C" int mlb_debug_fwd_marks(void* dev_buf) {
 }
 extern "C" int mlb_num_sms(mlb_handle h) { return h ? h->n_sms : 0; }
 extern "C" int mlb_last_kernel(mlb_handle h) { return h ? h->last_kernel : -1; }
-extern "C" int mlb_tc_resident_clusters(mlb_handle h) { return (h && h->tc) ? mlb_tc_max_clusters(h->tc) : 0; }
+extern "C" int mlb_tc_resident_clusters(mlb_handle h) { return (h && h->tc) ? mlb_tc_max_groups(h->tc) : 0; }
 extern "C" int mlb_device_error(mlb_handle h) { return h ? *reinterpret_cast<volatile int*>(h->err_flag_host) : -1; }
 
 static size_t fwd_smem_bytes(int L) {
@@ -938,7 +938,7 @@ extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream
     };
 
     // ---- large batches (and every batch of a model wider than the FFMA kernels cover): error-compensated TF32 on the
-    // tensor cores, persistent clusters over 64-row tiles (forward_tc.cu)
+    // tensor cores, persistent CTA groups over 64-row tiles (forward_tc.cu)
     const bool forced_ffma = (a->flags & (MLB_FWD_FORCE_TILE | MLB_FWD_FORCE_CLUSTER | MLB_FWD_FORCE_WIDE)) != 0 || a->rows_per_group != 0;
     if ((a->flags & MLB_FWD_FORCE_TC) && h->tc == nullptr)
         return fail("mlb_forward: the tensor-core kernel is not available for this model (linear_size % 256 != 0)");
@@ -946,9 +946,9 @@ extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream
     bool pick_tc = false;
     if (h->tc != nullptr && !forced_ffma && h->ffma_ok && a->n_rows > 64) {
         // measured wave times (calibrate()): tensor-core waves of row tiles against the better of FFMA clusters / row tiles
-        const int tc_cl = mlb_tc_clusters(h->tc, 1 << 30);
+        const int tc_groups = mlb_tc_groups(h->tc, 1 << 30);
         const long tc_tiles = (a->n_rows + mlb_tc_tile_rows() - 1) / mlb_tc_tile_rows();
-        const double t_tc = h->t_tc_wave * (double)((tc_tiles + tc_cl - 1) / tc_cl);
+        const double t_tc = h->t_tc_wave * (double)((tc_tiles + tc_groups - 1) / tc_groups);
         double t_ffma = 1e30;
         if (h->slab_dev != nullptr) t_ffma = h->t_cluster_wave * (double)(((a->n_rows + 15) / 16 + h->small_conc - 1) / h->small_conc);
         const int tmc = pick_rows_per_group(a->n_rows, h->n_sms);
@@ -959,9 +959,13 @@ extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream
         if (getenv("MLB_TC_MIN_ROWS")) pick_tc = a->n_rows >= h->tc_min_rows;
     }
     if (h->tc != nullptr && ((a->flags & MLB_FWD_FORCE_TC) || !h->ffma_ok || pick_tc)) {
-        arm_gather((unsigned)mlb_tc_clusters(h->tc, a->n_rows));  // one arrival per cluster leader
+        const unsigned done_before = h->gather_done_count;
+        arm_gather((unsigned)mlb_tc_groups(h->tc, a->n_rows));  // one arrival per group leader
         cudaError_t et = mlb_tc_launch(h->tc, p, st);
-        if (et != cudaSuccess) return fail(std::string("loco_forward_tc_kernel launch: ") + cudaGetErrorString(et));
+        if (et != cudaSuccess) {
+            h->gather_done_count = done_before;  // nothing ran
+            return fail(std::string("loco_forward_tc_kernel cooperative launch: ") + cudaGetErrorString(et));
+        }
         g_launches++;
         h->last_kernel = MLB_KERNEL_TC;
         return 0;

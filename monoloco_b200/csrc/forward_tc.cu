@@ -12,9 +12,12 @@
 //   weights      re-packed once per model: per GEMM op  [L/256 column tiles][K/16 k blocks][hi | lo][256 x 16]  (canonical
 //                K-major no-swizzle GMMA layout: core matrix 8 rows x 16 B, SBO 128 B, LBO rows x 16 B) -> a pipeline stage
 //                is two 1-D TMA bulk copies (8 KB of X planes + 32 KB of W planes), no tensor maps
-//   kernel       persistent thread-block clusters, L/256 CTAs each (4 at L = 1024).  A cluster owns a private workspace slot
-//                (input planes, two ping-pong activation plane sets, the fp32 residual; L2-resident for every cluster at
-//                once) and walks 64-row tiles.  CTA n owns output columns [256n, 256n + 256) of every layer.
+//   kernel       one cooperative, persistent grid of CTA groups, L/256 CTAs each (4 at L = 1024; floor(SMs / (L/256)) groups,
+//                33 on a 132-SM H100).  A group owns a private workspace slot (input planes, two ping-pong activation plane
+//                sets, the fp32 residual, the head partials, its barrier counter) and walks 64-row tiles.  CTA n owns output
+//                columns [256n, 256n + 256) of every layer.  Groups are not hardware clusters: clusters must fit one GPC,
+//                and only 30 four-CTA clusters fit an H100 at once (120 of 132 SMs; a 4096 batch then takes three rounds
+//                of tiles instead of two).
 //   per tile     prologue: thread = row: pre-process the raw keypoints (process.py:47-67 / 25-44) straight into hi / lo planes
 //                per layer: the producer warp streams the stages through a 4-slot ring (lane 0) and stages the layer's
 //                epilogue constants (the other lanes); consumer warpgroup c issues 2 k-steps x 3 wgmma (M 64, N 128, K 8)
@@ -23,9 +26,9 @@
 //                The summed accumulators go through shared memory (the idle ring) to a thread = (row, 64 columns) epilogue:
 //                folded BN / ReLU / dropout / residual, written straight into the next layer's hi / lo planes; narrow heads
 //                (w_aux, w_fin, MonolocoModel.w2) are accumulated on the CUDA cores from the same registers;
-//                barrier.cluster separates the layers
-//   tail         head partial sums -> CTA 0 through distributed shared memory -> decode_row -> stores (raw, decoded, xyz of
-//                the bbox-centre ray, fused all-gather peers), exactly the epilogue of the FFMA kernels (fwd_common.cuh).
+//                a group barrier (tc_group_sync: counter in global memory) separates the layers
+//   tail         head partial sums -> the group slot -> CTA 0 (fixed summation order) -> decode_row -> stores (raw, decoded,
+//                xyz of the bbox-centre ray, fused all-gather peers), exactly the epilogue of the FFMA kernels (fwd_common.cuh).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -44,7 +47,7 @@ constexpr uint32_t TC_A_PLANE = TCM * TCKB * 4;   // bytes of one X plane block 
 constexpr uint32_t TC_W_PLANE = TCN * TCKB * 4;   // bytes of one W plane block (256 output columns x 16 k)
 constexpr uint32_t TC_STAGE = 2 * TC_A_PLANE + 2 * TC_W_PLANE;   // 40 KB: X hi|lo + W hi|lo
 constexpr uint32_t TC_LBO_A = TCM * 16, TC_LBO_W = TCN * 16, TC_SBO = 128;
-constexpr int TC_MAX_CT = 8;       // column tiles = CTAs per cluster (L <= 2048)
+constexpr int TC_MAX_CT = 8;       // column tiles = CTAs per group (L <= 2048)
 constexpr int TC_HW = 16;          // head output columns in total (output_size <= 16)
 constexpr int TC_EPI = 256;        // consumer threads: 2 warpgroups (wgmma), then the epilogue, thread = (row, 64 columns)
 constexpr int TC_THREADS = TC_EPI + 32;   // + the producer warp (TMA ring, epilogue constants)
@@ -59,7 +62,7 @@ static_assert((size_t)4 * TC_MAX_CT * TCM * TC_HW * sizeof(float) <= TC_RING_BYT
 struct TcExtra {
     const float* wplanes[MLB_MAX_OPS];  // per GEMM op: [L/256 column tiles][n_kb][hi|lo][256 x 16]
     int n_kb[MLB_MAX_OPS];              // K blocks of 16 (K zero-padded)
-    float* ws;                          // workspace, one slot per cluster
+    float* ws;                          // workspace, one slot per group
     unsigned long long slot_floats;
     int n_tiles;                        // 64-row tiles of this launch
     // narrow heads: rows of all head ops concatenated (q = 0 .. n_head_rows-1)
@@ -100,14 +103,61 @@ __device__ __forceinline__ void tc_fence_regs(float* d) {
 #pragma unroll
     for (int i = 0; i < TCWN / 2; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ void tc_consumer_sync() { asm volatile("bar.sync 2, 256;" ::: "memory"); }   // the 2 consumer warpgroups
 __device__ __forceinline__ void tc_layer_sync() { asm volatile("bar.sync 1, 288;" ::: "memory"); }      // + the producer warp
-__device__ __forceinline__ uint32_t tc_cluster_id() {  // clusters are laid out along x: one cluster per blockIdx.x
-    return blockIdx.x;
+
+constexpr int TC_ERR_GROUP_TIMEOUT = 3;                       // the error word's "grid barrier" code
+constexpr unsigned long long TC_GROUP_TIMEOUT_NS = 20000000000ull;
+
+// Barrier over the nct = gridDim.y CTAs of one group (co-resident: cooperative launch).  The group's 64-bit counter only
+// ever grows: every CTA adds 1 per barrier, so barrier k of a launch completes at base + nct (k + 1), base being the counter
+// before the launch (tc_group_init).  A value left by an earlier launch is <= base and never satisfies a wait.  The CTA
+// barrier then the release-add order every thread's earlier stores before the arrival; the acquire poll then the CTA barrier
+// order the peers' stores before every thread's later accesses.  Bounded by %globaltimer: a missing arrival raises the error
+// word and turns this CTA's remaining waits into no-ops (target TC_GROUP_DEAD), so the kernel ends instead of hanging.
+// The state lives in shared memory: nothing of it stays live in registers across the layers.
+struct TcGroupBar {
+    unsigned long long* ctr;      // the group's counter (end of its workspace slot)
+    unsigned long long target;    // counter value that completes the next wait
+};
+constexpr unsigned long long TC_GROUP_DEAD = ~0ull;
+__device__ __forceinline__ void tc_group_wait(TcGroupBar* gb, int* err_flag) {   // thread 0
+    unsigned long long* ctr = gb->ctr;
+    asm volatile("red.release.gpu.global.add.u64 [%0], 1;" ::"l"(ctr) : "memory");
+    if (gb->target == TC_GROUP_DEAD) return;
+    const unsigned long long target = gb->target + gridDim.y;
+    gb->target = target;
+    unsigned long long t0 = 0;
+    for (unsigned spins = 1;; ++spins) {
+        unsigned long long v;
+        asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(ctr) : "memory");
+        if (v >= target) return;
+        if ((spins & 255u) == 0) {
+            unsigned long long t;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+            if (t0 == 0) {
+                t0 = t;
+            } else if (t - t0 > TC_GROUP_TIMEOUT_NS) {
+                if (err_flag) *reinterpret_cast<volatile int*>(err_flag) = TC_ERR_GROUP_TIMEOUT;
+                __threadfence_system();
+                gb->target = TC_GROUP_DEAD;
+                return;
+            }
+        }
+    }
+}
+__device__ __forceinline__ void tc_group_sync(TcGroupBar* gb, int* err_flag) {
+    __syncthreads();
+    if (threadIdx.x == 0) tc_group_wait(gb, err_flag);
+    __syncthreads();
+}
+// thread 0, before its first arrival: base = the counter before this launch.  Every earlier launch left it at a multiple of
+// nct, and the peers of this launch can be at most nct - 1 arrivals past it (barrier 0 needs this CTA's arrival).
+__device__ __forceinline__ void tc_group_init(TcGroupBar* gb, unsigned long long* ctr) {
+    unsigned long long v;
+    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(ctr) : "memory");
+    gb->ctr = ctr;
+    gb->target = v - v % gridDim.y;
 }
 
 // float offset of element (row r, k) inside one [tile_rows x 16] plane
@@ -131,8 +181,10 @@ __global__ void tc_pack_weights_kernel(const float* __restrict__ wt, float* __re
 }
 
 // profiling aid (mlb_debug_fwd_marks): CTA (0,0) stamps %globaltimer per layer of its first tile: thread 0 at [8g+0] layer start,
-// [8g+3] accumulators complete, [8g+4] epilogue done, [8g+5] cluster barrier passed; MMA lane at [8g+1] first stage landed,
-// [8g+2] all MMAs issued; producer lane at [8g+6] all stages issued
+// [8g+3] accumulators complete, [8g+4] epilogue done, [8g+5] group barrier passed; MMA lane at [8g+1] first stage landed,
+// [8g+2] all MMAs issued; producer lane at [8g+6] all stages issued.  Per tile t < 4 of group 0, thread 0: [128+4t] tile
+// start, [129+4t] prologue barrier passed, [130+4t] head partials gathered, [131+4t] rows stored.  Group barriers per tile:
+// one after the prologue, one per layer (the last one also publishes the head partials).
 __device__ unsigned long long* g_tc_marks = nullptr;
 __device__ __forceinline__ void tmark(unsigned long long* marks, int slot) {
     if (marks != nullptr) {
@@ -270,6 +322,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                                                                         const __grid_constant__ TcExtra ex) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t full[TCNST], empty[TCNST];
+    __shared__ TcGroupBar gbar;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int nt = blockIdx.y, nct = gridDim.y, L = p.L;
     const bool epi_thread = tid < TC_EPI, prod_warp = tid >= TC_EPI, prod_lane = tid == TC_EPI;
@@ -280,23 +333,24 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
     float* stg = reinterpret_cast<float*>(smem_raw);     // [64][TC_SLD] summed accumulators of the layer; aliases the idle ring
     float* hpart = reinterpret_cast<float*>(smem_raw);   // [4 nct][64][TC_HW] on CTA 0; aliases the idle ring
 
-    if (tid == 0) {
-        // every consumer warp releases a stage once its warpgroup's wgmma reading it have retired
-        for (int s = 0; s < TCNST; ++s) mbar_init(&full[s], 1), mbar_init(&empty[s], TC_EPI / 32);
-        mbar_fence_init();
-    }
-    __syncthreads();
-    tc_cluster_sync();  // every CTA of the cluster is resident before any remote shared-memory store can be issued
-
-    // this cluster's workspace slot
+    // this group's workspace slot
     int first_gemm = 0;
     while (p.ops[first_gemm].type != MLB_OP_GEMM) ++first_gemm;
     const int n_kb0 = ex.n_kb[first_gemm];
     const size_t plane = (size_t)TCM * TCKB;
-    float* slot = ex.ws + (size_t)tc_cluster_id() * ex.slot_floats;
+    float* slot = ex.ws + (size_t)blockIdx.x * ex.slot_floats;
     float* xin = slot;                                   // [n_kb0][hi|lo][64 x 16]
     float* xpl[2] = {xin + (size_t)n_kb0 * 2 * plane, xin + (size_t)n_kb0 * 2 * plane + (size_t)(L / TCKB) * 2 * plane};
     float* res = xpl[1] + (size_t)(L / TCKB) * 2 * plane;  // [L/4][64][4] fp32
+
+    if (tid == 0) {
+        // every consumer warp releases a stage once its warpgroup's wgmma reading it have retired
+        for (int s = 0; s < TCNST; ++s) mbar_init(&full[s], 1), mbar_init(&empty[s], TC_EPI / 32);
+        mbar_fence_init();
+        // after the residual: [4 nct][64][TC_HW] head partials of every CTA of the group, then the barrier counter
+        tc_group_init(&gbar, reinterpret_cast<unsigned long long*>(res + (size_t)TCM * L + (size_t)4 * nct * TCM * TC_HW));
+    }
+    __syncthreads();
 
     const float zm = p.z_met;
     const float k0 = p.kinv[0], k1 = p.kinv[1], k2 = p.kinv[2], k3 = p.kinv[3], k4 = p.kinv[4], k5 = p.kinv[5];
@@ -317,7 +371,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
     unsigned long long* marks = (blockIdx.x == 0 && blockIdx.y == 0 && (tid == 0 || prod_lane)) ? g_tc_marks : nullptr;
     unsigned it_p = 0, it_m = 0;  // stages issued / consumed so far (producer lane, consumer warpgroups)
     float acc_m[TCWN / 2], acc_c[TCWN / 2];   // this thread's wgmma fragments: main (a_hi.w_hi) and cross terms
-    for (int rb = (int)tc_cluster_id(); rb < ex.n_tiles; rb += (int)gridDim.x) {
+    for (int rb = (int)blockIdx.x; rb < ex.n_tiles; rb += (int)gridDim.x) {
+        unsigned long long* tmk = (tid == 0 && rb < 4 * (int)gridDim.x) ? marks : nullptr;   // group 0's first four tiles
+        const int tslot = 128 + 4 * (rb / (int)gridDim.x);
+        tmark(tmk, tslot);
         const int row = tid & (TCM - 1);      // epilogue threads: my row of the tile
         const int grow = rb * TCM + row;      // my detection
         const bool live = epi_thread && grow < p.n_rows;
@@ -325,7 +382,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
         float cenrow[4] = {0.f, 0.f, 0.f, 0.f};
 
         // ------------------------------------------------------------ prologue: network input of my row -> hi / lo planes
-        // every CTA of the cluster evaluates its row (cheap); CTA nt writes k blocks nt, nt + nct, ...
+        // every CTA of the group evaluates its row (cheap); CTA nt writes k blocks nt, nt + nct, ...
         if (row_owner) {
             float xr[KIN_MAX + 8];
 #pragma unroll
@@ -389,11 +446,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                 }
             }
         }
-        tc_cluster_sync();  // the input planes of this tile are complete (and the previous tile's tail is over everywhere)
-
-        float hacc[TC_HW];
-#pragma unroll
-        for (int q = 0; q < TC_HW; ++q) hacc[q] = 0.f;
+        tc_group_sync(&gbar, p.err_flag);   // the input planes of this tile are complete (and the previous tile's tail
+                                            // is over everywhere)
+        tmark(tmk, tslot + 1);
 
         int par = 0, site = 0, gi = 0;  // gi: GEMM ops done in this tile
         for (int oi = 0; oi < p.n_ops; ++oi) {
@@ -489,6 +544,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                 if (tid == 0) tmark(mk, 8 * gi + 3);
                 e.ccol0 = TCH * quarter, e.col0 = nt * TCN + TCH * quarter;
                 e.acc = stg + (size_t)row * TC_SLD + e.ccol0;
+                float hacc[TC_HW];   // head partial sums over my 64 columns; slots [off, off + nq) of the group fed here
+#pragma unroll
+                for (int q = 0; q < TC_HW; ++q) hacc[q] = 0.f;
                 if (!head_layer) {
                     if (e.add_res) tc_epilogue_cols<0, 0, true>(e, hacc);
                     else tc_epilogue_cols<0, 0, false>(e, hacc);
@@ -516,13 +574,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                         tc_epilogue_cols<4, 12, false>(e, hacc);
                     }
                 }
+                if (head_layer) {   // -> the group slot, [4 nt + quarter][row][TC_HW]; CTA 0 sums them after the last layer
+                    const int q4a = grp_off[hg] / 4, q4b = (grp_off[hg] + grp_nq[hg]) / 4;
+                    float4* dst = reinterpret_cast<float4*>(res + (size_t)TCM * L + ((size_t)(4 * nt + quarter) * TCM + row) * TC_HW);
+#pragma unroll
+                    for (int q4 = 0; q4 < TC_HW / 4; ++q4)
+                        if (q4 >= q4a && q4 < q4b) dst[q4] = make_float4(hacc[4 * q4], hacc[4 * q4 + 1], hacc[4 * q4 + 2], hacc[4 * q4 + 3]);
+                }
                 if (tid == 0) tmark(mk, 8 * gi + 4);
             }
             if (op.flags & MLB_F_DROPOUT) site++;
-            __syncwarp();
-            tc_cluster_sync();  // all column tiles of this row tile are written; the staging tile has been read
+            tc_group_sync(&gbar, p.err_flag);   // all column tiles of this row tile are written; the staging tile has been read
             if (tid == 0) tmark(mk, 8 * gi + 5);
-            // The planes this layer read are dead now (every CTA of the cluster is past its MMAs) and will be fully
+            // The planes this layer read are dead now (every CTA of the group is past its MMAs) and will be fully
             // rewritten before their next use: drop the dirty lines from L2 instead of letting them be written back to
             // HBM (discard.global.L2; without it the workspace churn was 255 MB of DRAM writes per batch of 4096).
             {
@@ -540,18 +604,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
             ++gi;
         }
 
-        // ------------------------------------------------------------ tail: head partials -> CTA 0 -> decode + stores
-        if (epi_thread) {
-            const uint32_t local = smem_u32(hpart + ((size_t)(4 * nt + quarter) * TCM + row) * TC_HW);
-            uint32_t remote;
-            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(0u));
-#pragma unroll
-            for (int q4 = 0; q4 < TC_HW / 4; ++q4)
-                asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(remote + 16u * q4), "f"(hacc[4 * q4]),
-                             "f"(hacc[4 * q4 + 1]), "f"(hacc[4 * q4 + 2]), "f"(hacc[4 * q4 + 3])
-                             : "memory");
+        // ------------------------------------------------------------ tail: head partials (slot) -> CTA 0 -> decode + stores
+        // the head layers wrote every CTA's partials to the slot; the last layer's group barrier ordered them before this point
+        if (nt == 0) {
+            // all partials into shared memory (the ring is idle) with independent 16-byte loads, then the fixed-order sum
+            const float4* src = reinterpret_cast<const float4*>(res + (size_t)TCM * L);   // [4 nct][64][TC_HW]
+            float4* dst = reinterpret_cast<float4*>(hpart);
+            for (int i = tid; i < nct * TCM * TC_HW; i += TC_THREADS) dst[i] = __ldcg(src + i);   // 4 nct x 64 x 16 floats
+            __syncthreads();
+            tmark(tmk, tslot + 2);
         }
-        tc_cluster_sync();
         if (nt == 0 && live && row_owner) {
             float o[OUT_LD];
 #pragma unroll
@@ -579,14 +641,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
             }
             __syncthreads();   // peer stores ordered before this CTA's arrival in gather_finish() (barrier + its fence)
         }
-        // the next tile's prologue ends with a cluster barrier: CTA 0 has finished reading hpart before any peer writes it
-        // again, and before its own producer refills the ring that hpart aliases (program order + fence.proxy.async)
+        tmark(tmk, tslot + 3);
+        // the next tile's prologue ends with a group barrier: CTA 0 has copied the partials before any peer writes them
+        // again, and has read its shared copy before its own producer refills the ring it aliases (program order +
+        // fence.proxy.async)
     }
     if (nt == 0) {
         __syncthreads();  // every storing thread has fenced its peer stores (store_row)
-        if (tid == 0) gather_finish(p);  // fused all-gather: one arrival per cluster leader
+        if (tid == 0) gather_finish(p);  // fused all-gather: one arrival per group leader
     }
-    tc_cluster_sync();  // no CTA exits while a peer may still address its shared memory
 }
 
 }  // namespace mlb
@@ -601,26 +664,14 @@ struct mlb_tc_state {
     int n_kb[MLB_MAX_OPS];
     float* ws;
     size_t slot_floats;
-    int max_clusters;
-    int nct;     // CTAs per cluster = L / 256
+    int max_groups;
+    int nct;     // CTAs per group = L / 256
 };
 
-// widths the tensor-core kernel covers: 256 output columns per CTA, clusters of up to 8 CTAs
+// widths the tensor-core kernel covers: 256 output columns per CTA, groups of up to 8 CTAs
 bool mlb_tc_supported(int L) { return L >= TCN && L % TCN == 0 && L / TCN <= TC_MAX_CT; }
 
-static void tc_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* at, int clusters, int nct, cudaStream_t st) {
-    memset(cfg, 0, sizeof(*cfg));
-    cfg->gridDim = dim3(clusters, nct);
-    cfg->blockDim = dim3(TC_THREADS);
-    cfg->dynamicSmemBytes = TC_SMEM_BYTES;
-    cfg->stream = st;
-    at->id = cudaLaunchAttributeClusterDimension;
-    at->val.clusterDim.x = 1, at->val.clusterDim.y = nct, at->val.clusterDim.z = 1;
-    cfg->attrs = at;
-    cfg->numAttrs = 1;
-}
-
-// pack the weight planes, size the workspace (one slot per co-resident cluster).  Returns nullptr + *err on failure.
+// pack the weight planes, size the workspace (one slot per co-resident group).  Returns nullptr + *err on failure.
 mlb_tc_state* mlb_tc_prepare(const float* blob_dev, const mlb_op* ops, int n_ops, int L, cudaStream_t st, cudaError_t* err) {
     mlb_tc_state* t = new mlb_tc_state();
     memset(t, 0, sizeof(*t));
@@ -636,21 +687,23 @@ mlb_tc_state* mlb_tc_prepare(const float* blob_dev, const mlb_op* ops, int n_ops
         if ((*err = cudaMalloc(&t->wplanes[i], fl * sizeof(float))) != cudaSuccess) return nullptr;
         tc_pack_weights_kernel<<<264, 256, 0, st>>>(blob_dev + ops[i].w_off, t->wplanes[i], ops[i].Kpad, L, t->n_kb[i]);
     }
-    cudaLaunchConfig_t cfg;
-    cudaLaunchAttribute at;
-    tc_config(&cfg, &at, 64, t->nct, st);
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, loco_forward_tc_kernel, &cfg) != cudaSuccess || n < 1) {
-        cudaGetLastError();
-        int dev = 0, sms = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        n = sms / t->nct / 2 > 0 ? sms / t->nct / 2 : 1;
+    // groups: as many as the co-resident CTAs hold (the cooperative launch needs all of them resident at once)
+    int dev = 0, sms = 0, per_sm = 0;
+    if ((*err = cudaGetDevice(&dev)) != cudaSuccess) return nullptr;
+    if ((*err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return nullptr;
+    if ((*err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, loco_forward_tc_kernel, TC_THREADS, TC_SMEM_BYTES)) != cudaSuccess)
+        return nullptr;
+    int n = per_sm * sms / t->nct;
+    if (n < 1) {
+        *err = cudaErrorCooperativeLaunchTooLarge;
+        return nullptr;
     }
     if (getenv("MLB_TC_CLUSTERS") && atoi(getenv("MLB_TC_CLUSTERS")) > 0 && atoi(getenv("MLB_TC_CLUSTERS")) < n) n = atoi(getenv("MLB_TC_CLUSTERS"));
-    t->max_clusters = n;
+    t->max_groups = n;
+    // slot: input planes, two plane sets, the fp32 residual, the head partials, the barrier counter (own 128-byte line)
     const size_t plane = (size_t)TCM * TCKB;
-    t->slot_floats = (size_t)t->n_kb[first] * 2 * plane + 2 * (size_t)(L / TCKB) * 2 * plane + (size_t)TCM * L;
+    t->slot_floats = (size_t)t->n_kb[first] * 2 * plane + 2 * (size_t)(L / TCKB) * 2 * plane + (size_t)TCM * L +
+                     (size_t)4 * t->nct * TCM * TC_HW + 32;
     if ((*err = cudaMalloc(&t->ws, (size_t)n * t->slot_floats * sizeof(float))) != cudaSuccess) return nullptr;
     if ((*err = cudaMemsetAsync(t->ws, 0, (size_t)n * t->slot_floats * sizeof(float), st)) != cudaSuccess) return nullptr;
     *err = cudaGetLastError();
@@ -671,11 +724,11 @@ void mlb_tc_free(mlb_tc_state* t) {
     delete t;
 }
 
-int mlb_tc_clusters(const mlb_tc_state* t, int n_rows) {
+int mlb_tc_groups(const mlb_tc_state* t, int n_rows) {
     const int tiles = (n_rows + TCM - 1) / TCM;
-    return tiles < t->max_clusters ? tiles : t->max_clusters;
+    return tiles < t->max_groups ? tiles : t->max_groups;
 }
-int mlb_tc_max_clusters(const mlb_tc_state* t) { return t->max_clusters; }
+int mlb_tc_max_groups(const mlb_tc_state* t) { return t->max_groups; }
 int mlb_tc_tile_rows() { return TCM; }
 
 cudaError_t mlb_tc_launch(const mlb_tc_state* t, const FwdParams& p, cudaStream_t st) {
@@ -700,7 +753,14 @@ cudaError_t mlb_tc_launch(const mlb_tc_state* t, const FwdParams& p, cudaStream_
         }
     }
     cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3(mlb_tc_groups(t, p.n_rows), t->nct);
+    cfg.blockDim = dim3(TC_THREADS);
+    cfg.dynamicSmemBytes = TC_SMEM_BYTES;
+    cfg.stream = st;
     cudaLaunchAttribute at;
-    tc_config(&cfg, &at, mlb_tc_clusters(t, p.n_rows), t->nct, st);
+    at.id = cudaLaunchAttributeCooperative;   // co-residency: the CTAs of a group spin on each other's arrivals
+    at.val.cooperative = 1;
+    cfg.attrs = &at, cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, loco_forward_tc_kernel, p, ex);
 }

@@ -90,8 +90,8 @@ class LocoEngine:
         return k, L_.KERNEL_NAMES.get(k, '?')
 
     def kernel_times(self):
-        """Per-wave kernel times measured at engine creation (ms) and the tensor-core cluster count: what mlb_forward's
-        kernel choice is based on."""
+        """Per-wave kernel times measured at engine creation (ms) and the tensor-core kernel's co-resident CTA group count
+        (`tc_resident_clusters`): what mlb_forward's kernel choice is based on."""
         t = (C.c_double * 4)()
         measured = self._lib.mlb_kernel_times(self._h, t)
         return {'measured': bool(measured), 'ffma_cluster_wave_ms': t[0], 'ffma_tile_wave_ms': '%.4f + %.4f * TM' % (t[1], t[2]),

@@ -1,5 +1,6 @@
-"""Timeline of CTA (0,0) inside the tensor-core forward kernel, first tile (mlb_debug_fwd_marks): per layer, us.
-    python tools/tc_marks.py [B]     (env: MLB_TC_N, MLB_TC_MC)"""
+"""Timeline of CTA (0,0) inside the tensor-core forward kernel (mlb_debug_fwd_marks), us: per layer of its first tile, then
+per tile of group 0 (prologue, layers, head partials, stores).
+    python tools/tc_marks.py [B]     (env: MLB_TC_CLUSTERS caps the group count)"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import ctypes as C
@@ -21,13 +22,24 @@ eng.forward(kps, **kw)
 torch.cuda.synchronize()
 L_.check(lib.mlb_debug_fwd_marks(C.c_void_p(0)), 'marks')
 m = buf.cpu().numpy().astype(np.int64)
-print('N=%s MC=%s B=%d resident clusters %d' % (os.environ.get('MLB_TC_N', 'auto'), os.environ.get('MLB_TC_MC', 'auto'), B,
-                                                 lib.mlb_tc_resident_clusters(eng._h)))
-t0 = m[0]
-for g in range(9):
-    s, first, issued, acc, epi, bar, prod, acc1 = m[8 * g:8 * g + 8]
+groups = lib.mlb_tc_resident_clusters(eng._h)
+tiles = (B + 63) // 64
+print('B=%d: %d tiles of 64 rows on %d co-resident CTA groups of 4 CTAs = %d tile round(s); %s' % (
+    B, tiles, groups, -(-tiles // groups), torch.cuda.get_device_name()))
+t0 = m[128]
+print('first tile of group 0, per layer (us from the layer start; layer start from the tile start):')
+for g in range(15):
+    s, first, issued, acc, epi, bar, prod = m[8 * g:8 * g + 7]
     if s == 0:
         break
-    print('layer %d @%7.1f: first stage +%5.1f | MMAs issued +%5.1f | accumulators done +%5.1f | epilogue end +%5.1f | '
-          'cluster barrier +%5.1f | producer done +%5.1f' % (g, (s - t0) / 1e3, (first - s) / 1e3, (issued - s) / 1e3, (acc - s) / 1e3,
-                                                             (epi - s) / 1e3, (bar - s) / 1e3, (prod - s) / 1e3))
+    print('  layer %d @%7.1f: first stage +%5.1f | MMAs issued +%5.1f | accumulators done +%5.1f | epilogue end +%5.1f | '
+          'group barrier +%5.1f | producer done +%5.1f' % (g, (s - t0) / 1e3, (first - s) / 1e3, (issued - s) / 1e3, (acc - s) / 1e3,
+                                                           (epi - s) / 1e3, (bar - s) / 1e3, (prod - s) / 1e3))
+print('tiles of group 0 (us from the kernel\'s first mark):')
+for t in range(4):
+    start, pro, heads, stored = m[128 + 4 * t:132 + 4 * t]
+    if start == 0:
+        break
+    print('  tile %d @%7.1f: prologue + barrier %5.1f | layers + head partials gathered %6.1f | rows stored +%5.1f | '
+          'tile %6.1f' % (t, (start - t0) / 1e3, (pro - start) / 1e3, (heads - pro) / 1e3, (stored - heads) / 1e3,
+                          (stored - start) / 1e3))
