@@ -155,6 +155,28 @@ int mlb_forward(mlb_handle h, const mlb_forward_args* args, void* stream);
  * (replaces net.py:92-93 `.to(device)` + process.py:261-263 `.detach().cpu()`). */
 int mlb_forward_host(mlb_handle h, const mlb_forward_args* host_args, void* stream);
 
+/* ---- many images in one forward launch, each with its own camera intrinsics (a video / multi-camera server,
+ * eval/generate_kitti.py over a split, MonStereo over a batch of image pairs).  Rows of all images are concatenated. */
+typedef struct mlb_image_batch {
+    int32_t n_img;            /* >= 1                                                                     */
+    int32_t reserved;
+    const int32_t* row_off;   /* [n_img + 1] device: network rows of image i are [row_off[i], row_off[i+1]);
+                                 row_off[0] == 0, row_off[n_img] == args->n_rows, non-decreasing            */
+    const int32_t* left_off;  /* stereo: [n_img + 1] device offsets into x (left poses), else NULL          */
+    const int32_t* right_off; /* stereo: [n_img + 1] device offsets into x_right, else NULL; image i owns
+                                 rows (l, r) at row_off[i] + l * nr_i + r, nr_i = right_off[i+1]-right_off[i] */
+    const float* kinv;        /* [n_img][9] device, K^-1 row-major fp32 (as mlb_post_args.kinv)            */
+} mlb_image_batch;
+
+/* mlb_forward with per-row intrinsics: row r uses the K^-1 of its image (args->kinv is ignored) for the pre-process and the
+ * bbox-centre ray of out_xyzc; in stereo, n_left / n_right are the totals over all images and each image pairs only its
+ * own poses (an image with zero left poses owns no rows).  input_kind MLB_IN_KPS or MLB_IN_KPS_STEREO; every flag keeps
+ * its meaning; n_gather must be 0.  Same kernel choice (on args->n_rows) as mlb_forward, and each row's outputs are those
+ * of the row run alone with its image's K on the same kernel, bit for bit (the counter-RNG dropout is keyed by the row
+ * index of the launch).  The offsets' contents are the caller's precondition; kernels clamp the image index and the pose
+ * indices they derive, so no read leaves x, x_right or kinv.  Device buffers, asynchronous on `stream`. */
+int mlb_forward_images(mlb_handle h, const mlb_forward_args* args, const mlb_image_batch* images, void* stream);
+
 /* pre-process only: [B,3,17] -> [B,34] (process.py:47-67), for callers such as
  * prep/preprocess_kitti.py:193 that never run the network.  Device buffers. */
 int mlb_preprocess(const float* kps, int n_rows, const float kinv[9], float z_met, int zero_center,
@@ -169,6 +191,15 @@ int mlb_preprocess(const float* kps, int n_rows, const float kinv[9], float z_me
 int mlb_stereo_filter(const float* raw, const float* dec, const float* xyzc, int n_left, int n_right, int out_size,
                       float* sel_raw, float* sel_dec, float* sel_xyzc, int32_t* sel_idx, int32_t* n_sel_dev,
                       int32_t* cnt_scratch, float* best_scratch, void* stream);
+/* The same filter over the rows of mlb_forward_images (stereo): `images` as given there (n_img, row_off, left_off,
+ * right_off; kinv unused), n_left / n_right the totals.  Kept rows are written image-major, each image in the row-major
+ * order of mlb_stereo_filter; sel_idx holds their row indices in `raw`, sel_img_off [n_img + 1] (device) the first
+ * kept row of every image and the total.  One warp per left pose, two launches, no host synchronisation;
+ * cnt_scratch / best_scratch [n_left]. */
+int mlb_stereo_filter_images(const float* raw, const float* dec, const float* xyzc, const mlb_image_batch* images, int n_left,
+                             int n_right, int out_size, float* sel_raw, float* sel_dec, float* sel_xyzc, int32_t* sel_idx,
+                             int32_t* n_sel_dev, int32_t* sel_img_off, int32_t* cnt_scratch, float* best_scratch,
+                             void* stream);
 
 /* ---- Loco.post_process for a BATCH of images on the device (net.py:164-248; utils/iou.py:6-29,44-64,87-101;
  * utils/camera.py:10-29,82-96,161-177).  Detections / ground truths of all images are concatenated; det_off / gt_off are

@@ -24,7 +24,7 @@ KERNEL_NAMES = {0: 'loco_forward_kernel (FFMA row tiles)', 1: 'loco_forward_clus
                 4: 'loco_forward_wide2_kernel (FFMA, 4-CTA clusters, K x N split)'}
 
 EXPORTS = ['mlb_create', 'mlb_update_weights', 'mlb_destroy', 'mlb_last_error', 'mlb_abi_version', 'mlb_num_sms', 'mlb_device_error', 'mlb_last_kernel', 'mlb_tc_resident_clusters', 'mlb_kernel_times',
-           'mlb_forward', 'mlb_forward_host', 'mlb_preprocess', 'mlb_stereo_filter', 'mlb_post_process', 'mlb_kitti_rows', 'mlb_decode', 'mlb_laplace_std', 'mlb_ipc_alloc', 'mlb_ipc_open', 'mlb_ipc_close', 'mlb_ipc_free', 'mlb_train_create', 'mlb_train_destroy',
+           'mlb_forward', 'mlb_forward_host', 'mlb_forward_images', 'mlb_preprocess', 'mlb_stereo_filter', 'mlb_stereo_filter_images', 'mlb_post_process', 'mlb_kitti_rows', 'mlb_decode', 'mlb_laplace_std', 'mlb_ipc_alloc', 'mlb_ipc_open', 'mlb_ipc_close', 'mlb_ipc_free', 'mlb_train_create', 'mlb_train_destroy',
            'mlb_train_forward', 'mlb_train_backward', 'mlb_train_step', 'mlb_train_phase_times', 'mlb_train_subphase_times',
            'mlb_adam_clip_step',
            'mlb_probe_ffma',
@@ -51,6 +51,11 @@ class MlbForwardArgs(C.Structure):
                 ('gather', C.c_void_p * MLB_MAX_PEERS), ('n_gather', C.c_int32), ('gather_rank', C.c_int32),
                 ('gather_row0', C.c_int64), ('gather_flags', C.c_void_p * MLB_MAX_PEERS), ('gather_epoch', C.c_uint32),
                 ('reserved0', C.c_int32)]
+
+
+class MlbImageBatch(C.Structure):
+    _fields_ = [('n_img', C.c_int32), ('reserved', C.c_int32), ('row_off', C.c_void_p), ('left_off', C.c_void_p),
+                ('right_off', C.c_void_p), ('kinv', C.c_void_p)]
 
 
 class MlbPostArgs(C.Structure):
@@ -111,9 +116,13 @@ def lib():
     l.mlb_kernel_times.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
     l.mlb_forward.argtypes = [C.c_void_p, C.POINTER(MlbForwardArgs), C.c_void_p]
     l.mlb_forward_host.argtypes = [C.c_void_p, C.POINTER(MlbForwardArgs), C.c_void_p]
+    l.mlb_forward_images.argtypes = [C.c_void_p, C.POINTER(MlbForwardArgs), C.POINTER(MlbImageBatch), C.c_void_p]
     l.mlb_preprocess.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_float), C.c_float, C.c_int, C.c_void_p, C.c_void_p]
     l.mlb_stereo_filter.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    l.mlb_stereo_filter_images.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(MlbImageBatch), C.c_int, C.c_int,
+                                           C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]
     l.mlb_post_process.argtypes = [C.POINTER(MlbPostArgs), C.c_void_p]
     l.mlb_kitti_rows.argtypes = [C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]

@@ -85,8 +85,9 @@ __device__ __forceinline__ void fmark(unsigned long long* marks, int slot) {
     }
 }
 
-template <int TM>
-__global__ void __launch_bounds__(MAX_THREADS, 1) loco_forward_kernel(const __grid_constant__ FwdParams p) {
+template <int TM, bool IMAGES>
+__global__ void __launch_bounds__(MAX_THREADS, 1) loco_forward_kernel(const __grid_constant__ FwdParams p,
+                                                                      const __grid_constant__ ImgParams ib) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int L = p.L;
@@ -150,6 +151,12 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_forward_kernel(const __gr
                     float v = 0.f;
                     if (r < rows_here && k < p.in_size) v = __ldg(p.x + (size_t)(row0 + r) * p.in_size + k);
                     xin[k * MP + smem_row(r, TM)] = v;
+                }
+            } else if constexpr (IMAGES) {
+                // one thread per row, with the row's own K^-1 and poses (fwd_common.cuh)
+                for (int r = tid; r < ROWS; r += nthreads) {
+                    const int sr = smem_row(r, TM);
+                    preprocess_row_images(p, ib, row0 + r, r < rows_here, cen + sr * 4, [&](int k, float v) { xin[k * MP + sr] = v; });
                 }
             } else {
                 const bool stereo = p.input_kind == MLB_IN_KPS_STEREO;
@@ -383,7 +390,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_forward_kernel(const __gr
                 const int sr = tid, grp = sr >> 4, i = sr & 15;
                 const int r = grp * TM + i;
                 if (i < TM && r < rows_here) {
-                    store_row(p, (size_t)row0 + r, outs + sr * OUT_LD, cen + sr * 4);
+                    store_row<IMAGES>(p, (size_t)row0 + r, outs + sr * OUT_LD, cen + sr * 4, nullptr, &ib);
                 }
             }
             consumer_sync(nthreads);
@@ -515,7 +522,8 @@ using namespace mlb;
 // forward_small.cu
 size_t mlb_small_smem_bytes(int L);
 cudaError_t mlb_small_pack(const float* blob, const mlb_op* ops, int n_ops, int L, float* slab, long long* slab_off, cudaStream_t st);
-cudaError_t mlb_small_launch(const FwdParams& p, const float* slab, const long long* slab_off, int n_clusters, cudaStream_t st);
+cudaError_t mlb_small_launch(const FwdParams& p, const ImgParams* ib, const float* slab, const long long* slab_off, int n_clusters,
+                             cudaStream_t st);
 int mlb_small_max_clusters(int L);
 // forward_wide2.cu
 size_t mlb_wide2_slab_floats(const mlb_op* ops, int n_ops, int L, long long* slab_off);
@@ -525,7 +533,7 @@ int mlb_wide2_epochs(const mlb_op* ops, int n_ops);
 size_t mlb_wide2_xg_pairs(int L);
 size_t mlb_wide2_hg_pairs(int L);
 cudaError_t mlb_wide2_set_marks(unsigned long long* ptr);
-cudaError_t mlb_wide2_launch(const FwdParams& p, const float* wslab, const long long* wslab_off, unsigned long long* xg,
+cudaError_t mlb_wide2_launch(const FwdParams& p, const ImgParams* ib, const float* wslab, const long long* wslab_off, unsigned long long* xg,
                              unsigned long long* hg, unsigned epoch_base, cudaStream_t st);
 // forward_tc.cu
 struct mlb_tc_state;
@@ -534,7 +542,7 @@ mlb_tc_state* mlb_tc_prepare(const float* blob_dev, const mlb_op* ops, int n_ops
 cudaError_t mlb_tc_repack(mlb_tc_state* t, const float* blob_dev, const mlb_op* ops, int n_ops, int L, cudaStream_t st);
 void mlb_tc_free(mlb_tc_state* t);
 int mlb_tc_groups(const mlb_tc_state* t, int n_rows);
-cudaError_t mlb_tc_launch(const mlb_tc_state* t, const FwdParams& p, cudaStream_t st);
+cudaError_t mlb_tc_launch(const mlb_tc_state* t, const FwdParams& p, const ImgParams* ib, cudaStream_t st);
 cudaError_t mlb_tc_set_marks(unsigned long long* ptr);
 int mlb_tc_max_groups(const mlb_tc_state* t);
 int mlb_tc_tile_rows();
@@ -544,7 +552,7 @@ cudaError_t mlb_wide_pack(const float* blob, const mlb_op* ops, int n_ops, int L
 bool mlb_wide_supported(int L, int n_sms);
 int mlb_wide_barriers(const mlb_op* ops, int n_ops);
 cudaError_t mlb_wide_set_marks(unsigned long long* ptr);
-cudaError_t mlb_wide_launch(const FwdParams& p, const float* wslab, const long long* wslab_off, float* xg, unsigned* bar,
+cudaError_t mlb_wide_launch(const FwdParams& p, const ImgParams* ib, const float* wslab, const long long* wslab_off, float* xg, unsigned* bar,
                             unsigned bar_base, cudaStream_t st);
 
 struct mlb_model {
@@ -846,16 +854,21 @@ static int pick_rows_per_group(int n_rows, int n_ctas) {
     return best;
 }
 
-template <int TM>
-static cudaError_t launch_fwd(const FwdParams& p, int grid, int threads, size_t smem, cudaStream_t st) {
-    cudaError_t e = cudaFuncSetAttribute(loco_forward_kernel<TM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+template <int TM, bool IMAGES>
+static cudaError_t launch_fwd(const FwdParams& p, const ImgParams& ib, int grid, int threads, size_t smem, cudaStream_t st) {
+    cudaError_t e = cudaFuncSetAttribute(loco_forward_kernel<TM, IMAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    loco_forward_kernel<TM><<<grid, threads, smem, st>>>(p);
+    loco_forward_kernel<TM, IMAGES><<<grid, threads, smem, st>>>(p, ib);
     return cudaGetLastError();
 }
+template <int TM>
+static cudaError_t launch_fwd(const FwdParams& p, const ImgParams* ib, int grid, int threads, size_t smem, cudaStream_t st) {
+    return ib ? launch_fwd<TM, true>(p, *ib, grid, threads, smem, st) : launch_fwd<TM, false>(p, ImgParams{}, grid, threads, smem, st);
+}
 
-extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream) {
-    if (!h || !a) return fail("mlb_forward: null argument");
+// mlb_forward (ib == nullptr: one K^-1 for every row) and mlb_forward_images (ib: per-image K^-1 and, in stereo, image-local
+// pairs).  The kernel choice is the same for both: it depends on the total row count only.
+static int forward_impl(mlb_handle h, const mlb_forward_args* a, const ImgParams* ib, void* stream) {
     if (a->n_rows < 0) return fail("mlb_forward: negative n_rows");
     if (a->n_gather < 0 || a->n_gather > MLB_MAX_PEERS) return fail("mlb_forward: n_gather out of range");
     const bool sync_gather = a->n_gather > 0 && a->gather_epoch != 0;
@@ -885,8 +898,9 @@ extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream
     if (a->input_kind == MLB_IN_KPS && d.input_size != 34) return fail("mlb_forward: MLB_IN_KPS needs a 34-d model");
     if (a->input_kind == MLB_IN_KPS_STEREO) {
         if (d.input_size != 68) return fail("mlb_forward: MLB_IN_KPS_STEREO needs a 68-d model");
-        if (!a->x_right || a->n_left < 1 || a->n_right < 1 || (long long)a->n_left * a->n_right != a->n_rows)
-            return fail("mlb_forward: stereo needs x_right and n_rows == n_left * n_right");
+        if (!a->x_right || a->n_left < 1 || a->n_right < 1 || (!ib && (long long)a->n_left * a->n_right != a->n_rows))
+            return fail(ib ? "mlb_forward_images: stereo needs x_right, n_left >= 1 and n_right >= 1"
+                           : "mlb_forward: stereo needs x_right and n_rows == n_left * n_right");
     }
     if (a->input_kind < MLB_IN_X || a->input_kind > MLB_IN_KPS_STEREO) return fail("mlb_forward: bad input_kind");
     if ((a->flags & MLB_FWD_ZERO_CENTER) && a->input_kind != MLB_IN_KPS) return fail("mlb_forward: zero_center needs MLB_IN_KPS");
@@ -961,7 +975,7 @@ extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream
     if (h->tc != nullptr && ((a->flags & MLB_FWD_FORCE_TC) || !h->ffma_ok || pick_tc)) {
         const unsigned done_before = h->gather_done_count;
         arm_gather((unsigned)mlb_tc_groups(h->tc, a->n_rows));  // one arrival per group leader
-        cudaError_t et = mlb_tc_launch(h->tc, p, st);
+        cudaError_t et = mlb_tc_launch(h->tc, p, ib, st);
         if (et != cudaSuccess) {
             h->gather_done_count = done_before;  // nothing ran
             return fail(std::string("loco_forward_tc_kernel cooperative launch: ") + cudaGetErrorString(et));
@@ -982,7 +996,7 @@ extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream
         const unsigned done_before = h->gather_done_count;
         arm_gather(1u);
         const unsigned base = h->wide2_epoch;
-        cudaError_t ew = mlb_wide2_launch(p, h->w2slab_dev, h->w2slab_off, h->wide2_xg, h->wide2_hg, base, st);
+        cudaError_t ew = mlb_wide2_launch(p, ib, h->w2slab_dev, h->w2slab_off, h->wide2_xg, h->wide2_hg, base, st);
         if (ew == cudaSuccess) {
             h->wide2_epoch = base + (unsigned)mlb_wide2_epochs(h->ops, d.n_ops);
             g_launches++;
@@ -1011,7 +1025,7 @@ extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream
             if (last_launch) arm_gather(1u);
             const unsigned base = h->wide_bar_count;
             h->wide_bar_count += (unsigned)mlb_wide_barriers(h->ops, d.n_ops) * (unsigned)(d.linear_size / 8);
-            cudaError_t ew = mlb_wide_launch(p, h->wslab_dev, h->wslab_off, h->wide_xg, h->wide_bar, base, st);
+            cudaError_t ew = mlb_wide_launch(p, ib, h->wslab_dev, h->wslab_off, h->wide_xg, h->wide_bar, base, st);
             if (ew != cudaSuccess) {
                 h->wide_bar_count = base;  // nothing ran: the device counters did not move
                 h->gather_done_count = done_before;
@@ -1045,7 +1059,7 @@ extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream
         if ((a->flags & MLB_FWD_FORCE_CLUSTER) || (a->rows_per_group == 0 && t_small < t_tile)) {
             p.n_tiles = n_clusters;
             arm_gather((unsigned)(n_clusters < conc ? n_clusters : conc));  // one arrival per cluster leader
-            cudaError_t es = mlb_small_launch(p, h->slab_dev, h->slab_off, n_clusters < conc ? n_clusters : conc, st);
+            cudaError_t es = mlb_small_launch(p, ib, h->slab_dev, h->slab_off, n_clusters < conc ? n_clusters : conc, st);
             if (es != cudaSuccess) return fail(std::string("loco_forward_cluster_kernel launch: ") + cudaGetErrorString(es));
             g_launches++;
             h->last_kernel = MLB_KERNEL_CLUSTER;
@@ -1073,16 +1087,37 @@ extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream
     arm_gather((unsigned)grid);  // every CTA owns >= 1 tile and arrives once
     cudaError_t e;
     switch (tm) {
-        case 8: e = launch_fwd<8>(p, grid, threads, smem, st); break;
-        case 10: e = launch_fwd<10>(p, grid, threads, smem, st); break;
-        case 12: e = launch_fwd<12>(p, grid, threads, smem, st); break;
-        case 14: e = launch_fwd<14>(p, grid, threads, smem, st); break;
-        default: e = launch_fwd<16>(p, grid, threads, smem, st); break;
+        case 8: e = launch_fwd<8>(p, ib, grid, threads, smem, st); break;
+        case 10: e = launch_fwd<10>(p, ib, grid, threads, smem, st); break;
+        case 12: e = launch_fwd<12>(p, ib, grid, threads, smem, st); break;
+        case 14: e = launch_fwd<14>(p, ib, grid, threads, smem, st); break;
+        default: e = launch_fwd<16>(p, ib, grid, threads, smem, st); break;
     }
     if (e != cudaSuccess) return fail(std::string("loco_forward_kernel launch: ") + cudaGetErrorString(e));
     g_launches++;
     h->last_kernel = MLB_KERNEL_TILE;
     return 0;
+}
+
+extern "C" int mlb_forward(mlb_handle h, const mlb_forward_args* a, void* stream) {
+    if (!h || !a) return fail("mlb_forward: null argument");
+    return forward_impl(h, a, nullptr, stream);
+}
+
+extern "C" int mlb_forward_images(mlb_handle h, const mlb_forward_args* a, const mlb_image_batch* b, void* stream) {
+    if (!h || !a || !b) return fail("mlb_forward_images: null argument");
+    if (b->n_img < 1) return fail("mlb_forward_images: n_img must be >= 1");
+    if (a->input_kind != MLB_IN_KPS && a->input_kind != MLB_IN_KPS_STEREO)
+        return fail("mlb_forward_images: input_kind must be MLB_IN_KPS or MLB_IN_KPS_STEREO (MLB_IN_X has no intrinsics)");
+    if (a->n_gather != 0) return fail("mlb_forward_images: the fused all-gather is not supported (n_gather must be 0)");
+    if (!b->row_off || !b->kinv) return fail("mlb_forward_images: row_off and kinv are required");
+    const bool stereo = a->input_kind == MLB_IN_KPS_STEREO;
+    if (stereo && (!b->left_off || !b->right_off)) return fail("mlb_forward_images: stereo needs left_off and right_off");
+    ImgParams ib;
+    ib.row_off = b->row_off, ib.left_off = stereo ? b->left_off : nullptr, ib.right_off = stereo ? b->right_off : nullptr;
+    ib.kinv = b->kinv;
+    ib.n_img = b->n_img, ib.n_left = a->n_left, ib.n_right = a->n_right;
+    return forward_impl(h, a, &ib, stream);
 }
 
 static int ensure(float** buf, size_t floats) {

@@ -76,8 +76,10 @@ struct SmallExtra {
     long long slab_off[MLB_MAX_OPS];   // float offset of each op's slab block
 };
 
+template <bool IMAGES>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 1)
-    loco_forward_cluster_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ SmallExtra ex) {
+    loco_forward_cluster_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ SmallExtra ex,
+                                const __grid_constant__ ImgParams ib) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int rank = (int)cluster_ctarank();
@@ -134,6 +136,12 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 1)
                 if (r < rows_here && k < p.in_size) v = __ldg(p.x + (size_t)(row0 + r) * p.in_size + k);
                 act[k * SR + r] = v;
             }
+        } else if constexpr (IMAGES) {
+            // one thread per row, with the row's own K^-1 and poses (fwd_common.cuh)
+            for (int r = tid; r < SR; r += 256)
+                preprocess_row_images(p, ib, row0 + r, r < rows_here, cen + r * 4, [&](int k, float v) { act[k * SR + r] = v; });
+            for (int idx = tid; idx < SR * (p.kpad0 - p.in_size); idx += 256)  // zero the K padding rows
+                act[(p.in_size + idx / SR) * SR + idx % SR] = 0.f;
         } else {
             const bool stereo = p.input_kind == MLB_IN_KPS_STEREO;
             if (tid < SR) {
@@ -333,7 +341,7 @@ __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(256, 1)
         if (rank == 0) {
             __syncthreads();
             if (tid < rows_here) {
-                store_row(p, (size_t)row0 + tid, outs + tid * OUT_LD, cen + tid * 4);
+                store_row<IMAGES>(p, (size_t)row0 + tid, outs + tid * OUT_LD, cen + tid * 4, nullptr, &ib);
             }
             __syncthreads();
         }
@@ -376,7 +384,7 @@ cudaError_t mlb_small_pack(const float* blob, const mlb_op* ops, int n_ops, int 
 // how many 8-CTA clusters of this kernel can be resident at once (GPC packing decides)
 int mlb_small_max_clusters(int L) {
     const size_t smem = mlb_small_smem_bytes(L);
-    if (cudaFuncSetAttribute(loco_forward_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 0;
+    if (cudaFuncSetAttribute(loco_forward_cluster_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 0;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(CL * 64);
@@ -388,20 +396,22 @@ int mlb_small_max_clusters(int L) {
     cfg.attrs = &at;
     cfg.numAttrs = 1;
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, loco_forward_cluster_kernel, &cfg) != cudaSuccess) {
+    if (cudaOccupancyMaxActiveClusters(&n, loco_forward_cluster_kernel<false>, &cfg) != cudaSuccess) {
         cudaGetLastError();
         return 0;
     }
     return n;
 }
 
-cudaError_t mlb_small_launch(const FwdParams& p, const float* slab, const long long* slab_off, int n_clusters, cudaStream_t st) {
+cudaError_t mlb_small_launch(const FwdParams& p, const ImgParams* ib, const float* slab, const long long* slab_off, int n_clusters,
+                             cudaStream_t st) {
     SmallExtra ex;
     ex.slab = slab;
     memcpy(ex.slab_off, slab_off, sizeof(ex.slab_off));
     const size_t smem = mlb_small_smem_bytes(p.L);
-    cudaError_t e = cudaFuncSetAttribute(loco_forward_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    auto kern = ib ? loco_forward_cluster_kernel<true> : loco_forward_cluster_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    loco_forward_cluster_kernel<<<n_clusters * CL, 256, smem, st>>>(p, ex);
+    kern<<<n_clusters * CL, 256, smem, st>>>(p, ex, ib ? *ib : ImgParams{});
     return cudaGetLastError();
 }

@@ -318,8 +318,10 @@ __device__ __forceinline__ void tc_epilogue_cols(const TcEpi& e, float* hacc) {
     }
 }
 
+template <bool IMAGES>
 __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __grid_constant__ FwdParams p,
-                                                                        const __grid_constant__ TcExtra ex) {
+                                                                        const __grid_constant__ TcExtra ex,
+                                                                        const __grid_constant__ ImgParams ib) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     __shared__ __align__(8) uint64_t full[TCNST], empty[TCNST];
     __shared__ TcGroupBar gbar;
@@ -392,6 +394,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
 #pragma unroll
                     for (int k = 0; k < KIN_MAX; ++k)
                         if (k < p.in_size) xr[k] = __ldg(p.x + (size_t)grow * p.in_size + k);
+                } else if constexpr (IMAGES) {
+                    // the row's own K^-1 and poses (fwd_common.cuh)
+                    preprocess_row_images(p, ib, grow, true, cenrow, [&](int k, float v) { xr[k] = v; });
                 } else {
                     const bool stereo = p.input_kind == MLB_IN_KPS_STEREO;
                     const float* kp = p.x + (size_t)(stereo ? grow / p.n_right : grow) * 51;
@@ -625,7 +630,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                 for (int t = 0; t < 4 * nct; ++t) s += hpart[((size_t)t * TCM + row) * TC_HW + slot];  // fixed order: deterministic
                 o[ex.head_col[q]] = s + __ldg(p.blob + ex.head_b[q]);
             }
-            store_row(p, (size_t)grow, o, cenrow, p.n_gather ? hw + (size_t)row * MLB_GATHER_LD : nullptr);
+            store_row<IMAGES>(p, (size_t)grow, o, cenrow, p.n_gather ? hw + (size_t)row * MLB_GATHER_LD : nullptr, &ib);
         }
         if (nt == 0 && p.n_gather) {
             // fused all-gather: the tile's rows ([<=64][20] floats, contiguous in every gather buffer) leave as coalesced
@@ -676,7 +681,9 @@ mlb_tc_state* mlb_tc_prepare(const float* blob_dev, const mlb_op* ops, int n_ops
     mlb_tc_state* t = new mlb_tc_state();
     memset(t, 0, sizeof(*t));
     t->nct = L / TCN;
-    *err = cudaFuncSetAttribute(loco_forward_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_BYTES);
+    *err = cudaFuncSetAttribute(loco_forward_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_BYTES);
+    if (*err == cudaSuccess)
+        *err = cudaFuncSetAttribute(loco_forward_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_BYTES);
     if (*err != cudaSuccess) { delete t; return nullptr; }
     int first = -1;
     for (int i = 0; i < n_ops; ++i) {
@@ -691,7 +698,7 @@ mlb_tc_state* mlb_tc_prepare(const float* blob_dev, const mlb_op* ops, int n_ops
     int dev = 0, sms = 0, per_sm = 0;
     if ((*err = cudaGetDevice(&dev)) != cudaSuccess) return nullptr;
     if ((*err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return nullptr;
-    if ((*err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, loco_forward_tc_kernel, TC_THREADS, TC_SMEM_BYTES)) != cudaSuccess)
+    if ((*err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, loco_forward_tc_kernel<false>, TC_THREADS, TC_SMEM_BYTES)) != cudaSuccess)
         return nullptr;
     int n = per_sm * sms / t->nct;
     if (n < 1) {
@@ -731,7 +738,7 @@ int mlb_tc_groups(const mlb_tc_state* t, int n_rows) {
 int mlb_tc_max_groups(const mlb_tc_state* t) { return t->max_groups; }
 int mlb_tc_tile_rows() { return TCM; }
 
-cudaError_t mlb_tc_launch(const mlb_tc_state* t, const FwdParams& p, cudaStream_t st) {
+cudaError_t mlb_tc_launch(const mlb_tc_state* t, const FwdParams& p, const ImgParams* ib, cudaStream_t st) {
     TcExtra ex;
     memset(&ex, 0, sizeof(ex));
     for (int i = 0; i < MLB_MAX_OPS; ++i) ex.wplanes[i] = t->wplanes[i], ex.n_kb[i] = t->n_kb[i];
@@ -762,5 +769,8 @@ cudaError_t mlb_tc_launch(const mlb_tc_state* t, const FwdParams& p, cudaStream_
     at.id = cudaLaunchAttributeCooperative;   // co-residency: the CTAs of a group spin on each other's arrivals
     at.val.cooperative = 1;
     cfg.attrs = &at, cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, loco_forward_tc_kernel, p, ex);
+    // the multi-image instantiation has the same shared memory and register budget (__launch_bounds__), so the same
+    // per-SM occupancy and group count
+    if (ib) return cudaLaunchKernelEx(&cfg, loco_forward_tc_kernel<true>, p, ex, *ib);
+    return cudaLaunchKernelEx(&cfg, loco_forward_tc_kernel<false>, p, ex, ImgParams{});
 }

@@ -54,9 +54,10 @@ __device__ __forceinline__ void wmark(unsigned long long* marks, int slot) {
     }
 }
 
-template <int R>  // row slots of the tile: 16 or 32
+template <int R, bool IMAGES>  // row slots of the tile: 16 or 32
 __global__ void __launch_bounds__(WNT, 1) loco_forward_wide_kernel(const __grid_constant__ FwdParams p,
-                                                                   const __grid_constant__ WideExtra ex) {
+                                                                   const __grid_constant__ WideExtra ex,
+                                                                   const __grid_constant__ ImgParams ib) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     constexpr int S = 2 * WNT / R;  // k-subsets: thread (s, row pair q) accumulates k = s, s + S, s + 2S, ... for rows 2q, 2q+1
     const int tid = threadIdx.x;
@@ -118,7 +119,7 @@ __global__ void __launch_bounds__(WNT, 1) loco_forward_wide_kernel(const __grid_
 
     const int row0 = p.row_base;
     const int rows_here = min(R, p.n_rows - row0);  // a single tile
-    stage_input_tile(p, row0, rows_here, R, R, act, cen, tid, WNT, [] { __syncthreads(); });
+    stage_input_tile<IMAGES>(p, ib, row0, rows_here, R, R, act, cen, tid, WNT, [] { __syncthreads(); });
     __syncthreads();
     if (cta == 0 && p.out_x != nullptr && p.input_kind != MLB_IN_X) {
         for (int idx = tid; idx < rows_here * p.in_size; idx += WNT) {
@@ -235,7 +236,7 @@ __global__ void __launch_bounds__(WNT, 1) loco_forward_wide_kernel(const __grid_
     // ---- decode + store (CTA 0, one thread per row)
     __syncthreads();
     wmark(marks, 2 + 4 * n_gemm);
-    if (tid < rows_here) store_row(p, (size_t)row0 + tid, outs + tid * OUT_LD, cen + tid * 4);
+    if (tid < rows_here) store_row<IMAGES>(p, (size_t)row0 + tid, outs + tid * OUT_LD, cen + tid * 4, nullptr, &ib);
     if (p.n_gather) {
         __syncthreads();
         if (tid == 0) gather_finish(p);  // CTA 0 is the only storing CTA of this kernel
@@ -303,11 +304,11 @@ cudaError_t mlb_wide_pack(const float* blob, const mlb_op* ops, int n_ops, int L
 bool mlb_wide_supported(int L, int n_sms) {
     if (L % 128 != 0 || L / WC > n_sms) return false;
     int occ = 0;
-    if (cudaFuncSetAttribute(loco_forward_wide_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide_smem<32>(L)) != cudaSuccess)
+    if (cudaFuncSetAttribute(loco_forward_wide_kernel<32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide_smem<32>(L)) != cudaSuccess)
         return false;
-    if (cudaFuncSetAttribute(loco_forward_wide_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide_smem<16>(L)) != cudaSuccess)
+    if (cudaFuncSetAttribute(loco_forward_wide_kernel<16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide_smem<16>(L)) != cudaSuccess)
         return false;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, loco_forward_wide_kernel<32>, WNT, wide_smem<32>(L)) != cudaSuccess || occ < 1)
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, loco_forward_wide_kernel<32, false>, WNT, wide_smem<32>(L)) != cudaSuccess || occ < 1)
         return false;
     return true;
 }
@@ -319,21 +320,22 @@ int mlb_wide_barriers(const mlb_op* ops, int n_ops) {
     return n;
 }
 
-cudaError_t mlb_wide_launch(const FwdParams& p, const float* wslab, const long long* wslab_off, float* xg, unsigned* bar,
-                            unsigned bar_base, cudaStream_t st) {
+template <int R, bool IMAGES>
+static cudaError_t wide_launch_r(void** args, int L, cudaStream_t st) {
+    // (the opt-in shared-memory size is a per-function, per-process attribute: set it for THIS model's width on every launch)
+    cudaError_t e = cudaFuncSetAttribute(loco_forward_wide_kernel<R, IMAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide_smem<R>(L));
+    if (e != cudaSuccess) return e;
+    return cudaLaunchCooperativeKernel((void*)loco_forward_wide_kernel<R, IMAGES>, dim3(L / WC), dim3(WNT), args, wide_smem<R>(L), st);
+}
+
+cudaError_t mlb_wide_launch(const FwdParams& p, const ImgParams* ib, const float* wslab, const long long* wslab_off, float* xg,
+                            unsigned* bar, unsigned bar_base, cudaStream_t st) {
     WideExtra ex;
     ex.wslab = wslab;
     for (int i = 0; i < MLB_MAX_OPS; ++i) ex.wslab_off[i] = i < p.n_ops ? wslab_off[i] : 0;
     ex.xg = xg, ex.bar = bar, ex.bar_base = bar_base;
-    void* args[] = {(void*)&p, (void*)&ex};
-    const int grid = p.L / WC;
-    // (the opt-in shared-memory size is a per-function, per-process attribute: set it for THIS model's width on every launch)
-    if (p.n_rows - p.row_base <= 16) {
-        cudaError_t e = cudaFuncSetAttribute(loco_forward_wide_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide_smem<16>(p.L));
-        if (e != cudaSuccess) return e;
-        return cudaLaunchCooperativeKernel((void*)loco_forward_wide_kernel<16>, dim3(grid), dim3(WNT), args, wide_smem<16>(p.L), st);
-    }
-    cudaError_t e = cudaFuncSetAttribute(loco_forward_wide_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide_smem<32>(p.L));
-    if (e != cudaSuccess) return e;
-    return cudaLaunchCooperativeKernel((void*)loco_forward_wide_kernel<32>, dim3(grid), dim3(WNT), args, wide_smem<32>(p.L), st);
+    ImgParams ibv = ib ? *ib : ImgParams{};
+    void* args[] = {(void*)&p, (void*)&ex, (void*)&ibv};
+    if (p.n_rows - p.row_base <= 16) return ib ? wide_launch_r<16, true>(args, p.L, st) : wide_launch_r<16, false>(args, p.L, st);
+    return ib ? wide_launch_r<32, true>(args, p.L, st) : wide_launch_r<32, false>(args, p.L, st);
 }

@@ -80,8 +80,10 @@ __device__ __forceinline__ void w2mark(unsigned long long* marks, int slot) {
     }
 }
 
+template <bool IMAGES>
 __global__ void __cluster_dims__(W2_CL, 1, 1) __launch_bounds__(W2_NT, 2)
-    loco_forward_wide2_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ Wide2Extra ex) {
+    loco_forward_wide2_kernel(const __grid_constant__ FwdParams p, const __grid_constant__ Wide2Extra ex,
+                              const __grid_constant__ ImgParams ib) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     constexpr int R = W2_R;
     const int tid = threadIdx.x;
@@ -139,7 +141,7 @@ __global__ void __cluster_dims__(W2_CL, 1, 1) __launch_bounds__(W2_NT, 2)
     const int row0 = p.row_base;
     const int rows_here = min(R, p.n_rows - row0);
     // network input: every CTA evaluates the tile's pre-process; the first layer's K (<= 72) lies in slice 0
-    stage_input_tile(p, row0, rows_here, R, R, act, cen, tid, W2_NT, [] { __syncthreads(); });
+    stage_input_tile<IMAGES>(p, ib, row0, rows_here, R, R, act, cen, tid, W2_NT, [] { __syncthreads(); });
     __syncthreads();
     if (blockIdx.x == 0 && p.out_x != nullptr && p.input_kind != MLB_IN_X) {
         for (int idx = tid; idx < rows_here * p.in_size; idx += W2_NT) {
@@ -378,7 +380,7 @@ __global__ void __cluster_dims__(W2_CL, 1, 1) __launch_bounds__(W2_NT, 2)
     }
     __syncthreads();
     w2mark(marks, 3 + 4 * n_gemm);
-    if (tid < rows_here) store_row(p, (size_t)row0 + tid, outs + tid * OUT_LD, cen + tid * 4);
+    if (tid < rows_here) store_row<IMAGES>(p, (size_t)row0 + tid, outs + tid * OUT_LD, cen + tid * 4, nullptr, &ib);
     if (p.n_gather) {
         __syncthreads();
         if (tid == 0) gather_finish(p);   // CTA 0 is the only storing CTA of this kernel
@@ -431,7 +433,7 @@ bool mlb_wide2_supported(const mlb_op* ops, int n_ops, int L, int out_size, int 
     if (L % 128 != 0 || L / W2_FC > n_sms || out_size > W2_HQ) return false;
     for (int i = 0; i < n_ops; ++i)
         if (ops[i].type == MLB_OP_GEMM && (ops[i].flags & MLB_F_IN_XIN) && ops[i].Kpad > L / W2_CL) return false;
-    if (cudaFuncSetAttribute(loco_forward_wide2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide2_smem(L)) != cudaSuccess) {
+    if (cudaFuncSetAttribute(loco_forward_wide2_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide2_smem(L)) != cudaSuccess) {
         cudaGetLastError();
         return false;
     }
@@ -439,7 +441,7 @@ bool mlb_wide2_supported(const mlb_op* ops, int n_ops, int L, int out_size, int 
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(L / W2_FC), cfg.blockDim = dim3(W2_NT), cfg.dynamicSmemBytes = wide2_smem(L);
     int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, loco_forward_wide2_kernel, &cfg) != cudaSuccess || n < L / W2_NC) {
+    if (cudaOccupancyMaxActiveClusters(&n, loco_forward_wide2_kernel<false>, &cfg) != cudaSuccess || n < L / W2_NC) {
         cudaGetLastError();
         return false;
     }
@@ -455,15 +457,16 @@ int mlb_wide2_epochs(const mlb_op* ops, int n_ops) {   // epochs one launch cons
 size_t mlb_wide2_xg_pairs(int L) { return (size_t)3 * L * W2_R; }
 size_t mlb_wide2_hg_pairs(int L) { return (size_t)(L / W2_NC) * W2_HQ * W2_R; }
 
-cudaError_t mlb_wide2_launch(const FwdParams& p, const float* wslab, const long long* wslab_off, unsigned long long* xg,
-                             unsigned long long* hg, unsigned epoch_base, cudaStream_t st) {
+cudaError_t mlb_wide2_launch(const FwdParams& p, const ImgParams* ib, const float* wslab, const long long* wslab_off,
+                             unsigned long long* xg, unsigned long long* hg, unsigned epoch_base, cudaStream_t st) {
     Wide2Extra ex;
     ex.wslab = wslab;
     for (int i = 0; i < MLB_MAX_OPS; ++i) ex.wslab_off[i] = i < p.n_ops ? wslab_off[i] : 0;
     ex.xg = xg, ex.hg = hg, ex.epoch_base = epoch_base;
     // the opt-in shared-memory size is a per-function attribute of the PROCESS: another handle with a narrower model may have
     // lowered it since this one was created
-    cudaError_t e = cudaFuncSetAttribute(loco_forward_wide2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide2_smem(p.L));
+    auto kern = ib ? loco_forward_wide2_kernel<true> : loco_forward_wide2_kernel<false>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide2_smem(p.L));
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
@@ -472,5 +475,5 @@ cudaError_t mlb_wide2_launch(const FwdParams& p, const float* wslab, const long 
     at.id = cudaLaunchAttributeCooperative;   // co-residency of all clusters: they spin on each other's outputs
     at.val.cooperative = 1;
     cfg.attrs = &at, cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, loco_forward_wide2_kernel, p, ex);
+    return cudaLaunchKernelEx(&cfg, kern, p, ex, ib ? *ib : ImgParams{});
 }

@@ -38,6 +38,99 @@ struct FwdParams {
 
 enum { ERR_GATHER_TIMEOUT = 4 };
 
+// Many images in one launch (mlb_forward_images): the image description, passed as a trailing kernel parameter so that
+// no FwdParams field moves.  Only the <IMAGES = true> instantiations read it; the others compile as before.
+struct ImgParams {
+    const int* row_off;    // [n_img + 1] network rows of image i: [row_off[i], row_off[i + 1])
+    const int* left_off;   // stereo: [n_img + 1] offsets into x (left poses)
+    const int* right_off;  // stereo: [n_img + 1] offsets into x_right
+    const float* kinv;     // [n_img][9] K^-1 row-major
+    int n_img, n_left, n_right;  // n_left / n_right: totals over all images (clamp bounds)
+};
+
+// Image of network row `grow`: the last i with row_off[i] <= grow, clamped to [0, n_img) whatever the offsets hold.
+__device__ __forceinline__ int image_of_row(const ImgParams& ib, int grow) {
+    int lo = 0, hi = ib.n_img - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (__ldg(ib.row_off + mid) <= grow) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
+// Where row `grow` reads its inputs: its image's K^-1 and its left (and right) pose, clamped inside x / x_right.
+// Stereo row (l, r) of image i is row_off[i] + l * nr_i + r (the image-local form of the all-vs-all rows l * R + r).
+struct RowSrc {
+    const float* kinv;
+    int li, ri;
+};
+__device__ __forceinline__ RowSrc row_source(const ImgParams& ib, int grow, bool stereo) {
+    const int i = image_of_row(ib, grow);
+    RowSrc s;
+    s.kinv = ib.kinv + (size_t)i * 9;
+    s.li = grow, s.ri = 0;
+    if (stereo) {
+        const int loc = grow - __ldg(ib.row_off + i);
+        const int nr = max(1, __ldg(ib.right_off + i + 1) - __ldg(ib.right_off + i));
+        s.li = min(max(__ldg(ib.left_off + i) + loc / nr, 0), ib.n_left - 1);
+        s.ri = min(max(__ldg(ib.right_off + i) + loc % nr, 0), ib.n_right - 1);
+    }
+    return s;
+}
+
+// Pre-process of ONE row of a multi-image launch by one thread (process.py:25-67 with the row's own K^-1): the same
+// expressions in the same order as the single-K staging code, so a row's network input is bit-identical to that of the
+// row run alone with its image's K.  put(k, v) stores input feature k; cen receives (u_c, v_c, x_c * z_met, y_c * z_met).
+// A row beyond the batch (live == false) stores zeros.
+template <typename Put>
+__device__ __forceinline__ void preprocess_row_images(const FwdParams& p, const ImgParams& ib, int grow, bool live, float* cen,
+                                                      Put put) {
+    const bool stereo = p.input_kind == MLB_IN_KPS_STEREO;
+    if (!live) {
+        cen[0] = cen[1] = cen[2] = cen[3] = 0.f;
+#pragma unroll
+        for (int k = 0; k < 34; ++k) put(k, 0.f);
+        if (stereo) {
+#pragma unroll
+            for (int k = 34; k < 68; ++k) put(k, 0.f);
+        }
+        return;
+    }
+    const RowSrc s = row_source(ib, grow, stereo);
+    const float zm = p.z_met;
+    const float k0 = __ldg(s.kinv + 0), k1 = __ldg(s.kinv + 1), k2 = __ldg(s.kinv + 2);
+    const float k3 = __ldg(s.kinv + 3), k4 = __ldg(s.kinv + 4), k5 = __ldg(s.kinv + 5);
+    const float* kp = p.x + (size_t)s.li * 51;
+    const float* kr = p.xr + (size_t)s.ri * 51;
+    float umin = __ldg(kp), umax = umin, vmin = __ldg(kp + 17), vmax = vmin;
+    for (int j = 1; j < 17; ++j) {
+        const float u = __ldg(kp + j), v = __ldg(kp + 17 + j);
+        umin = fminf(umin, u), umax = fmaxf(umax, u);
+        vmin = fminf(vmin, v), vmax = fmaxf(vmax, v);
+    }
+    const float uc = __fadd_rn(__fdiv_rn(__fsub_rn(umax, umin), 2.f), umin);  // camera.py:82-86
+    const float vc = __fadd_rn(__fdiv_rn(__fsub_rn(vmax, vmin), 2.f), vmin);
+    const float cx = (uc * k0 + vc * k1 + k2) * zm, cy = (uc * k3 + vc * k4 + k5) * zm;
+    cen[0] = uc, cen[1] = vc, cen[2] = cx, cen[3] = cy;
+    const bool zc = (p.flags & MLB_FWD_ZERO_CENTER) != 0;
+#pragma unroll
+    for (int j = 0; j < 17; ++j) {
+        const float u = __ldg(kp + j), v = __ldg(kp + 17 + j);
+        float xl = (u * k0 + v * k1 + k2) * zm;  // camera.py:26-27, rows 0/1 of [u v 1] K^-T
+        float yl = (u * k3 + v * k4 + k5) * zm;
+        if (stereo) {
+            const float ur = __ldg(kr + j), vr = __ldg(kr + 17 + j);
+            put(34 + 2 * j, xl - (ur * k0 + vr * k1 + k2) * zm);  // process.py:41 cat(l, l - r)
+            put(35 + 2 * j, yl - (ur * k3 + vr * k4 + k5) * zm);
+        } else if (zc) {
+            xl -= cx;  // process.py:61-62
+            yl -= cy;
+        }
+        put(2 * j, xl);
+        put(2 * j + 1, yl);
+    }
+}
+
 // Called by ONE thread of every CTA that stored gather rows, after a CTA barrier that follows those stores.  No per-thread
 // fence is needed (one fence.sc.sys per storing thread cost 20 us per launch): the barrier orders the CTA's stores before
 // this thread, its gpu-scope fence + arrival (release pattern) and the last arriver's system-scope fence + st.release.sys
@@ -112,10 +205,11 @@ __device__ __forceinline__ void decode_row(int kind, int out_size, const float* 
 // Pre-process of one row tile into the k-major input tile xin[k][ld] (process.py:25-67 preprocess_monoloco /
 // preprocess_monstereo, camera.py:26-27 pixel_to_camera, camera.py:82-86 bbox centre), rows [row0, row0 + rows_here) ->
 // slots 0.., remaining slots and the K padding rows zero.  cen[slot] = (u_c, v_c, x_c * z_met, y_c * z_met).
-// `sync` is the caller's barrier over the `nthreads` participating threads.
-template <typename Sync>
-__device__ __forceinline__ void stage_input_tile(const FwdParams& p, int row0, int rows_here, int slots, int ld, float* xin,
-                                                 float* cen, int tid, int nthreads, Sync sync) {
+// `sync` is the caller's barrier over the `nthreads` participating threads.  IMAGES: one thread per row, with the row's
+// own K^-1 and poses (preprocess_row_images).
+template <bool IMAGES, typename Sync>
+__device__ __forceinline__ void stage_input_tile(const FwdParams& p, const ImgParams& ib, int row0, int rows_here, int slots,
+                                                 int ld, float* xin, float* cen, int tid, int nthreads, Sync sync) {
     const float zm = p.z_met;
     const float k0 = p.kinv[0], k1 = p.kinv[1], k2 = p.kinv[2], k3 = p.kinv[3], k4 = p.kinv[4], k5 = p.kinv[5];
     if (p.input_kind == MLB_IN_X) {
@@ -125,6 +219,13 @@ __device__ __forceinline__ void stage_input_tile(const FwdParams& p, int row0, i
             if (r < rows_here && k < p.in_size) v = __ldg(p.x + (size_t)(row0 + r) * p.in_size + k);
             xin[k * ld + r] = v;
         }
+        return;
+    }
+    if constexpr (IMAGES) {
+        for (int r = tid; r < slots; r += nthreads)
+            preprocess_row_images(p, ib, row0 + r, r < rows_here, cen + r * 4, [&](int k, float v) { xin[k * ld + r] = v; });
+        for (int idx = tid; idx < slots * (p.kpad0 - p.in_size); idx += nthreads)  // zero the K padding rows
+            xin[(p.in_size + idx / slots) * ld + idx % slots] = 0.f;
         return;
     }
     const bool stereo = p.input_kind == MLB_IN_KPS_STEREO;
@@ -181,8 +282,10 @@ __device__ __forceinline__ void stage_input_tile(const FwdParams& p, int row0, i
 // One decoded row -> the caller's outputs (raw, decoded, xyz of the bbox-centre ray, fused all-gather peers).
 // gather_stage != nullptr: instead of storing the gather row to the peers itself, the row ([MLB_GATHER_LD] floats) is left
 // there (shared memory) and the caller ships the whole tile with coalesced stores.
+// IMAGES: the bbox-centre ray uses the K^-1 of the row's image (looked up here, once per row) instead of p.kinv.
+template <bool IMAGES = false>
 __device__ __forceinline__ void store_row(const FwdParams& p, size_t grow, const float* o, const float* cen_row,
-                                          float* gather_stage = nullptr) {
+                                          float* gather_stage = nullptr, const ImgParams* ib = nullptr) {
     for (int k = 0; k < p.out_size; ++k) p.out_raw[grow * p.out_size + k] = o[k];
     float x, y, z, d, bi, yaw_p, yaw_o, aux;
     decode_row(p.decode_kind, p.out_size, o, x, y, z, d, bi, yaw_p, yaw_o, aux);
@@ -205,9 +308,17 @@ __device__ __forceinline__ void store_row(const FwdParams& p, size_t grow, const
     if (p.out_xyzc != nullptr && p.input_kind != MLB_IN_X) {
         // net.py:195,213: xy_centers = pixel_to_camera(uv_centers, kk, 1); xyz_from_distance(d, centre)
         const float uc = cen_row[0], vc = cen_row[1];
-        const float cx = uc * p.kinv[0] + vc * p.kinv[1] + p.kinv[2];
-        const float cy = uc * p.kinv[3] + vc * p.kinv[4] + p.kinv[5];
-        const float cz = uc * p.kinv[6] + vc * p.kinv[7] + p.kinv[8];
+        float cx, cy, cz;
+        if constexpr (IMAGES) {
+            const float* kv = ib->kinv + (size_t)image_of_row(*ib, (int)grow) * 9;
+            cx = uc * __ldg(kv + 0) + vc * __ldg(kv + 1) + __ldg(kv + 2);
+            cy = uc * __ldg(kv + 3) + vc * __ldg(kv + 4) + __ldg(kv + 5);
+            cz = uc * __ldg(kv + 6) + vc * __ldg(kv + 7) + __ldg(kv + 8);
+        } else {
+            cx = uc * p.kinv[0] + vc * p.kinv[1] + p.kinv[2];
+            cy = uc * p.kinv[3] + vc * p.kinv[4] + p.kinv[5];
+            cz = uc * p.kinv[6] + vc * p.kinv[7] + p.kinv[8];
+        }
         const float den = sqrtf(__fadd_rn(__fadd_rn(1.f, __fmul_rn(cx, cx)), __fmul_rn(cy, cy)));
         const float px = __fdiv_rn(__fmul_rn(cx, d), den), py = __fdiv_rn(__fmul_rn(cy, d), den),
                     pz = __fdiv_rn(__fmul_rn(cz, d), den);

@@ -24,20 +24,51 @@ namespace mlb {
 // monstereo arg-max filter: one warp per left pose.
 //   pass 1: cnt[l] = #{r : aux[l][r] >= max_r aux[l][r]}   (0 if any NaN: torch.max propagates NaN -> mask all False)
 //   pass 2: offset = sum(cnt[0..l)), ordered compaction of the kept rows (row-major: ties keep their order)
+// Left poses are global over the images of the CSR, whose images are consecutive in both the left poses and the rows, so
+// the kept rows come out image-major; one image (left_off == nullptr) is the all-vs-all batch l * n_right + r.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_max(float v) {
     for (int s = 16; s > 0; s >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, s));
     return v;
 }
 
-__global__ void stereo_count_kernel(const float* __restrict__ raw, int n_left, int n_right, int out_size,
+struct StereoCsr {
+    const int32_t* row_off;    // [n_img + 1] (mlb_image_batch), or nullptr: one image
+    const int32_t* left_off;
+    const int32_t* right_off;
+    int32_t* sel_img_off;      // [n_img + 1] out, or nullptr
+    int n_img;
+};
+
+// rows of left pose l: [row0, row0 + nr), image-local pairs (l, r) -> row0 + r; bounded by the image's rows
+__device__ __forceinline__ void left_rows(const StereoCsr& c, int l, int n_right, size_t& row0, int& nr) {
+    if (c.left_off == nullptr) {
+        row0 = (size_t)l * n_right, nr = n_right;
+        return;
+    }
+    int lo = 0, hi = c.n_img - 1;  // image: last i with left_off[i] <= l, clamped
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (c.left_off[mid] <= l) lo = mid; else hi = mid - 1;
+    }
+    const int first = c.row_off[lo], end = c.row_off[lo + 1];
+    nr = max(0, c.right_off[lo + 1] - c.right_off[lo]);
+    const long long r0 = (long long)first + (long long)(l - c.left_off[lo]) * nr;
+    if (r0 < first || r0 + nr > end) nr = 0;  // offsets inconsistent with each other: read nothing
+    row0 = (size_t)max(r0, 0ll);
+}
+
+__global__ void stereo_count_kernel(const float* __restrict__ raw, StereoCsr csr, int n_left, int n_right, int out_size,
                                     int32_t* __restrict__ cnt, float* __restrict__ best_out) {
     const int l = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (l >= n_left) return;
-    const float* v = raw + (size_t)l * n_right * out_size + (out_size - 1);
+    size_t row0;
+    int nr;
+    left_rows(csr, l, n_right, row0, nr);
+    const float* v = raw + row0 * out_size + (out_size - 1);
     float best = -INFINITY;
     bool nan = false;
-    for (int r = lane; r < n_right; r += 32) {
+    for (int r = lane; r < nr; r += 32) {
         const float x = v[(size_t)r * out_size];
         nan |= (x != x);
         best = fmaxf(best, x);  // fmaxf ignores NaN; NaN rows are handled through `nan`
@@ -46,13 +77,13 @@ __global__ void stereo_count_kernel(const float* __restrict__ raw, int n_left, i
     nan = __any_sync(0xffffffffu, nan);
     int c = 0;
     if (!nan)
-        for (int r = lane; r < n_right; r += 32) c += v[(size_t)r * out_size] >= best;
+        for (int r = lane; r < nr; r += 32) c += v[(size_t)r * out_size] >= best;
     for (int s = 16; s > 0; s >>= 1) c += __shfl_xor_sync(0xffffffffu, c, s);
     if (lane == 0) cnt[l] = c, best_out[l] = best;
 }
 
 __global__ void stereo_scatter_kernel(const float* __restrict__ raw, const float* __restrict__ dec, const float* __restrict__ xyzc,
-                                      int n_left, int n_right, int out_size, const int32_t* __restrict__ cnt,
+                                      StereoCsr csr, int n_left, int n_right, int out_size, const int32_t* __restrict__ cnt,
                                       const float* __restrict__ best_in, float* __restrict__ sel_raw, float* __restrict__ sel_dec,
                                       float* __restrict__ sel_xyzc, int32_t* __restrict__ sel_idx, int32_t* __restrict__ n_sel) {
     const int l = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -62,16 +93,30 @@ __global__ void stereo_scatter_kernel(const float* __restrict__ raw, const float
     for (int s = 16; s > 0; s >>= 1) off += __shfl_xor_sync(0xffffffffu, off, s);
     const int mine = cnt[l];
     if (l == n_left - 1 && lane == 0) *n_sel = off + mine;
+    if (csr.sel_img_off != nullptr && lane == 0) {
+        // every image whose left poses start at l starts at `off`; after the last pose, the remaining entries get the total
+        int j = 0, hi = csr.n_img;  // first j with left_off[j] >= l
+        while (j < hi) {
+            const int mid = (j + hi) >> 1;
+            if (csr.left_off[mid] < l) j = mid + 1; else hi = mid;
+        }
+        for (; j <= csr.n_img && csr.left_off[j] == l; ++j) csr.sel_img_off[j] = off;
+        if (l == n_left - 1)
+            for (; j <= csr.n_img; ++j) csr.sel_img_off[j] = off + mine;
+    }
     if (mine == 0) return;
     const float best = best_in[l];
-    const float* v = raw + (size_t)l * n_right * out_size + (out_size - 1);
-    for (int r0 = 0; r0 < n_right; r0 += 32) {
+    size_t row0;
+    int nr;
+    left_rows(csr, l, n_right, row0, nr);
+    const float* v = raw + row0 * out_size + (out_size - 1);
+    for (int r0 = 0; r0 < nr; r0 += 32) {
         const int r = r0 + lane;
-        const bool keep = r < n_right && v[(size_t)r * out_size] >= best;
+        const bool keep = r < nr && v[(size_t)r * out_size] >= best;
         const unsigned m = __ballot_sync(0xffffffffu, keep);
         if (keep) {
             const int pos = off + __popc(m & ((1u << lane) - 1u));
-            const size_t src = (size_t)l * n_right + r;
+            const size_t src = row0 + r;
             sel_idx[pos] = (int32_t)src;
             for (int k = 0; k < out_size; ++k) sel_raw[(size_t)pos * out_size + k] = raw[src * out_size + k];
             if (dec != nullptr && sel_dec != nullptr)
@@ -255,20 +300,47 @@ static int pfail(const std::string& msg) {
         if (e_ != cudaSuccess) return pfail(std::string(#call) + ": " + cudaGetErrorString(e_));  \
     } while (0)
 
-extern "C" int mlb_stereo_filter(const float* raw, const float* dec, const float* xyzc, int n_left, int n_right, int out_size,
-                                 float* sel_raw, float* sel_dec, float* sel_xyzc, int32_t* sel_idx, int32_t* n_sel_dev,
-                                 int32_t* cnt_scratch, float* best_scratch, void* stream) {
-    if (!raw || !sel_raw || !sel_idx || !n_sel_dev || !cnt_scratch || !best_scratch || n_left < 1 || n_right < 1 || out_size < 1)
-        return pfail("mlb_stereo_filter: bad argument");
+static int stereo_filter_launch(const float* raw, const float* dec, const float* xyzc, const StereoCsr& c, int n_left, int n_right,
+                                int out_size, float* sel_raw, float* sel_dec, float* sel_xyzc, int32_t* sel_idx, int32_t* n_sel_dev,
+                                int32_t* cnt_scratch, float* best_scratch, cudaStream_t st) {
     const int wpb = 4, grid = (n_left + wpb - 1) / wpb;
-    cudaStream_t st = (cudaStream_t)stream;
-    stereo_count_kernel<<<grid, wpb * 32, 0, st>>>(raw, n_left, n_right, out_size, cnt_scratch, best_scratch);
-    stereo_scatter_kernel<<<grid, wpb * 32, 0, st>>>(raw, dec, xyzc, n_left, n_right, out_size, cnt_scratch, best_scratch, sel_raw,
+    stereo_count_kernel<<<grid, wpb * 32, 0, st>>>(raw, c, n_left, n_right, out_size, cnt_scratch, best_scratch);
+    stereo_scatter_kernel<<<grid, wpb * 32, 0, st>>>(raw, dec, xyzc, c, n_left, n_right, out_size, cnt_scratch, best_scratch, sel_raw,
                                                      sel_dec, sel_xyzc, sel_idx, n_sel_dev);
     PCU(cudaGetLastError());
     mlb_count_launch();
     mlb_count_launch();
     return 0;
+}
+
+extern "C" int mlb_stereo_filter(const float* raw, const float* dec, const float* xyzc, int n_left, int n_right, int out_size,
+                                 float* sel_raw, float* sel_dec, float* sel_xyzc, int32_t* sel_idx, int32_t* n_sel_dev,
+                                 int32_t* cnt_scratch, float* best_scratch, void* stream) {
+    if (!raw || !sel_raw || !sel_idx || !n_sel_dev || !cnt_scratch || !best_scratch || n_left < 1 || n_right < 1 || out_size < 1)
+        return pfail("mlb_stereo_filter: bad argument");
+    const StereoCsr one = {nullptr, nullptr, nullptr, nullptr, 1};
+    return stereo_filter_launch(raw, dec, xyzc, one, n_left, n_right, out_size, sel_raw, sel_dec, sel_xyzc, sel_idx, n_sel_dev,
+                                cnt_scratch, best_scratch, (cudaStream_t)stream);
+}
+
+extern "C" int mlb_stereo_filter_images(const float* raw, const float* dec, const float* xyzc, const mlb_image_batch* b, int n_left,
+                                        int n_right, int out_size, float* sel_raw, float* sel_dec, float* sel_xyzc, int32_t* sel_idx,
+                                        int32_t* n_sel_dev, int32_t* sel_img_off, int32_t* cnt_scratch, float* best_scratch,
+                                        void* stream) {
+    if (!b || !b->row_off || !b->left_off || !b->right_off || b->n_img < 1 || !sel_img_off || !n_sel_dev || n_left < 0 ||
+        n_right < 0 || out_size < 1)
+        return pfail("mlb_stereo_filter_images: bad argument");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_left == 0) {  // no left poses in any image: nothing kept
+        PCU(cudaMemsetAsync(sel_img_off, 0, (size_t)(b->n_img + 1) * sizeof(int32_t), st));
+        PCU(cudaMemsetAsync(n_sel_dev, 0, sizeof(int32_t), st));
+        return 0;
+    }
+    if (!raw || !sel_raw || !sel_idx || !cnt_scratch || !best_scratch || n_right < 1)
+        return pfail("mlb_stereo_filter_images: bad argument");
+    const StereoCsr c = {b->row_off, b->left_off, b->right_off, sel_img_off, b->n_img};
+    return stereo_filter_launch(raw, dec, xyzc, c, n_left, n_right, out_size, sel_raw, sel_dec, sel_xyzc, sel_idx, n_sel_dev,
+                                cnt_scratch, best_scratch, st);
 }
 
 extern "C" int mlb_post_process(const mlb_post_args* a, void* stream) {

@@ -29,6 +29,49 @@ def kinv_from_kk(kk):
     return v
 
 
+def kinv_images(kk_list):
+    """K^-1 of every image (kinv_from_kk), packed [n_img, 9] fp32 as mlb_image_batch.kinv expects."""
+    return np.stack([kinv_from_kk(kk) for kk in kk_list]).astype(np.float32).reshape(len(kk_list), 9)
+
+
+def image_offsets(counts):
+    """Per-image counts -> int32 CSR offsets [n_img + 1] (0, n_0, n_0 + n_1, ...)."""
+    off = np.zeros(len(counts) + 1, dtype=np.int64)
+    np.cumsum(np.asarray(counts, dtype=np.int64), out=off[1:])
+    if off[-1] > np.iinfo(np.int32).max:
+        raise ValueError("more than 2^31 - 1 rows")
+    return off.astype(np.int32)
+
+
+def check_image_batch(row_off, n_rows, left_off=None, right_off=None, n_left=None, n_right=None):
+    """Host check of the offsets of mlb_forward_images (the kernels only clamp): int32 [n_img + 1] arrays, each starting at 0,
+    non-decreasing and ending at its total; in stereo, image i owns (left_off[i+1] - left_off[i]) * (right_off[i+1] -
+    right_off[i]) rows.  Returns the offsets as int32 numpy arrays."""
+    def csr(name, off, total):
+        off = np.asarray(off, dtype=np.int64).reshape(-1)
+        if off.size < 2:
+            raise ValueError("%s: at least one image needed (n_img + 1 >= 2 offsets)" % name)
+        if off[0] != 0 or off[-1] != total or (np.diff(off) < 0).any():
+            raise ValueError("%s must start at 0, be non-decreasing and end at %d" % (name, total))
+        if total > np.iinfo(np.int32).max:
+            raise ValueError("%s: more than 2^31 - 1 rows" % name)
+        return off.astype(np.int32)
+    row_off = csr('row_off', row_off, n_rows)
+    if left_off is None:
+        return row_off, None, None
+    left_off, right_off = csr('left_off', left_off, n_left), csr('right_off', right_off, n_right)
+    if not (left_off.size == right_off.size == row_off.size):
+        raise ValueError("row_off, left_off and right_off must have n_img + 1 entries each")
+    if (np.diff(row_off.astype(np.int64)) != np.diff(left_off.astype(np.int64)) * np.diff(right_off.astype(np.int64))).any():
+        raise ValueError("stereo: image i must own n_left_i * n_right_i rows")
+    return row_off, left_off, right_off
+
+
+def _upload(arr, device):
+    """Small host array -> device tensor through torch's pinned-memory cache (asynchronous, stream-ordered)."""
+    return torch.from_numpy(np.ascontiguousarray(arr)).pin_memory().to(device, non_blocking=True)
+
+
 class LocoEngine:
     def __init__(self, state_dict, p_dropout=0.2, device=None):
         if not torch.cuda.is_available():
@@ -116,9 +159,7 @@ class LocoEngine:
         x = x.contiguous()
         a = L_.MlbForwardArgs()
         a.input_kind = kind
-        a.flags = (L_.FWD_ZERO_CENTER if zero_center else 0) | (L_.FWD_DROPOUT if dropout else 0) | \
-                  {None: 0, 'tile': L_.FWD_FORCE_TILE, 'cluster': L_.FWD_FORCE_CLUSTER, 'wide': L_.FWD_FORCE_WIDE,
-                   'tc': L_.FWD_FORCE_TC, 'wide2': L_.FWD_FORCE_WIDE2}[kernel]
+        a.flags = self._flags(zero_center, dropout, kernel)
         if kind == L_.IN_KPS_STEREO:
             x_right = x_right.contiguous()
             n_left, n_right = x.shape[0], x_right.shape[0]
@@ -134,8 +175,31 @@ class LocoEngine:
             a.z_met = 10.0
         a.n_rows = B
         a.rows_per_group = rows_per_group
-        out = {'raw': torch.empty((B, self.output_size), dtype=torch.float32, device=self.device)}
         a.x = x.data_ptr()
+        out = self._outputs(a, B, want_dec, want_xyzc, want_x, drop_mask, drop_seed)
+        if gather_ptrs:
+            a.n_gather = len(gather_ptrs)
+            for i, ptr in enumerate(gather_ptrs):
+                a.gather[i] = ptr
+            a.gather_row0 = int(gather_row0)
+            if gather_flags:  # device-side completion protocol (include/monoloco_b200.h: gather_epoch)
+                for i, ptr in enumerate(gather_flags):
+                    a.gather_flags[i] = ptr
+                a.gather_rank = int(gather_rank)
+                a.gather_epoch = int(gather_epoch) & 0xFFFFFFFF
+        if B > 0 or (gather_ptrs and gather_flags and gather_epoch):  # an empty shard still signals its epoch
+            L_.check(self._lib.mlb_forward(self._h, C.byref(a), self._stream()), 'mlb_forward')
+        return out
+
+    @staticmethod
+    def _flags(zero_center, dropout, kernel):
+        return (L_.FWD_ZERO_CENTER if zero_center else 0) | (L_.FWD_DROPOUT if dropout else 0) | \
+            {None: 0, 'tile': L_.FWD_FORCE_TILE, 'cluster': L_.FWD_FORCE_CLUSTER, 'wide': L_.FWD_FORCE_WIDE,
+             'tc': L_.FWD_FORCE_TC, 'wide2': L_.FWD_FORCE_WIDE2}[kernel]
+
+    def _outputs(self, a, B, want_dec, want_xyzc, want_x, drop_mask, drop_seed):
+        """Device output tensors of a forward of B rows, their pointers and the dropout arguments set in `a`."""
+        out = {'raw': torch.empty((B, self.output_size), dtype=torch.float32, device=self.device)}
         a.out_raw = out['raw'].data_ptr()
         if want_dec:
             out['dec'] = torch.empty((B, 8), dtype=torch.float32, device=self.device)
@@ -151,18 +215,57 @@ class LocoEngine:
             drop_mask = drop_mask.contiguous()
             a.drop_mask = drop_mask.data_ptr()
         a.drop_seed = int(drop_seed)
-        if gather_ptrs:
-            a.n_gather = len(gather_ptrs)
-            for i, ptr in enumerate(gather_ptrs):
-                a.gather[i] = ptr
-            a.gather_row0 = int(gather_row0)
-            if gather_flags:  # device-side completion protocol (include/monoloco_b200.h: gather_epoch)
-                for i, ptr in enumerate(gather_flags):
-                    a.gather_flags[i] = ptr
-                a.gather_rank = int(gather_rank)
-                a.gather_epoch = int(gather_epoch) & 0xFFFFFFFF
-        if B > 0 or (gather_ptrs and gather_flags and gather_epoch):  # an empty shard still signals its epoch
-            L_.check(self._lib.mlb_forward(self._h, C.byref(a), self._stream()), 'mlb_forward')
+        return out
+
+    def _image_batch(self, row_off, kk_list, B, left_off=None, right_off=None, n_left=None, n_right=None):
+        """Checked host offsets + K^-1 per image (kk_list None: no intrinsics, the stereo filter) -> (mlb_image_batch,
+        device tensors it points into)."""
+        row_off, left_off, right_off = check_image_batch(row_off, B, left_off, right_off, n_left, n_right)
+        n_img = row_off.size - 1
+        if kk_list is not None and len(kk_list) != n_img:
+            raise ValueError("one camera matrix per image: %d matrices for %d images" % (len(kk_list), n_img))
+        offs = _upload(np.concatenate([row_off] + ([left_off, right_off] if left_off is not None else [])), self.device)
+        kinv = _upload(kinv_images(kk_list), self.device) if kk_list is not None else None
+        ib = L_.MlbImageBatch()
+        ib.n_img = n_img
+        ib.row_off = offs.data_ptr()
+        if left_off is not None:
+            ib.left_off = offs.data_ptr() + 4 * (n_img + 1)
+            ib.right_off = offs.data_ptr() + 8 * (n_img + 1)
+        ib.kinv = kinv.data_ptr() if kinv is not None else None
+        return ib, (offs, kinv)
+
+    def forward_images(self, x, row_off, kk_list, kind=L_.IN_KPS, x_right=None, left_off=None, right_off=None,
+                       want_dec=True, want_xyzc=False, want_x=False, zero_center=False, dropout=False, drop_mask=None,
+                       drop_seed=0, kernel=None):
+        """Many images in ONE forward launch, each with its own camera matrix (mlb_forward_images).
+        x: keypoints of all images concatenated (CUDA [B,3,17]; stereo: left poses [n_left,3,17] and x_right [n_right,3,17]).
+        row_off (and in stereo left_off / right_off): host int CSR offsets [n_img + 1], checked here; kk_list: one K per
+        image.  Returns the dict of CUDA tensors forward() returns, rows image-major (stereo: image-local pairs l * nr + r)."""
+        assert x.is_cuda and x.dtype == torch.float32
+        if kind not in (L_.IN_KPS, L_.IN_KPS_STEREO):
+            raise ValueError("forward_images: keypoint inputs only (MLB_IN_X carries no camera intrinsics)")
+        x = x.contiguous()
+        a = L_.MlbForwardArgs()
+        a.input_kind = kind
+        a.flags = self._flags(zero_center, dropout, kernel)
+        if kind == L_.IN_KPS_STEREO:
+            if x_right is None or left_off is None or right_off is None:
+                raise ValueError("forward_images: stereo needs x_right, left_off and right_off")
+            x_right = x_right.contiguous()
+            a.n_left, a.n_right = x.shape[0], x_right.shape[0]
+            a.x_right = x_right.data_ptr()
+            B = int(np.asarray(row_off)[-1])
+            ib, keep = self._image_batch(row_off, kk_list, B, left_off, right_off, a.n_left, a.n_right)
+        else:
+            B = x.shape[0]
+            ib, keep = self._image_batch(row_off, kk_list, B)
+        a.n_rows = B
+        a.z_met = 10.0
+        a.x = x.data_ptr()
+        out = self._outputs(a, B, want_dec, want_xyzc, want_x, drop_mask, drop_seed)
+        if B > 0:
+            L_.check(self._lib.mlb_forward_images(self._h, C.byref(a), C.byref(ib), self._stream()), 'mlb_forward_images')
         return out
 
     def forward_host(self, x, x_right=None, kk=None, kind=L_.IN_X, want_dec=True, want_xyzc=False, out=None,
@@ -226,6 +329,37 @@ class LocoEngine:
         res = (sel_raw[:n], (sel_dec[:n] if dec is not None else None), sel_idx[:n])
         return res + (sel_xyzc[:n],) if xyzc is not None else res
 
+    def stereo_filter_images(self, raw, dec, row_off, left_off, right_off, xyzc=None, trim=True):
+        """process.py:307-327 per image over the rows of a stereo forward_images (mlb_stereo_filter_images): kept rows
+        image-major, each image in the order stereo_filter gives it.  Returns a dict of CUDA tensors sel_raw, sel_dec,
+        sel_idx (row indices into raw), sel_xyzc, n_sel [1] and sel_img_off [n_img + 1]; trim=True cuts them to the
+        kept rows and turns sel_img_off into a host list (one synchronisation)."""
+        n_left, n_right = int(np.asarray(left_off)[-1]), int(np.asarray(right_off)[-1])
+        B = raw.shape[0]
+        ib, keep = self._image_batch(row_off, None, B, left_off, right_off, n_left, n_right)
+        out = {'sel_raw': torch.empty_like(raw), 'sel_dec': torch.empty_like(dec) if dec is not None else None,
+               'sel_xyzc': torch.empty_like(xyzc) if xyzc is not None else None,
+               'sel_idx': torch.empty((B,), dtype=torch.int32, device=self.device),
+               'n_sel': torch.empty((1,), dtype=torch.int32, device=self.device),
+               'sel_img_off': torch.empty((ib.n_img + 1,), dtype=torch.int32, device=self.device)}
+        cnt = torch.empty((max(n_left, 1),), dtype=torch.int32, device=self.device)
+        best = torch.empty((max(n_left, 1),), dtype=torch.float32, device=self.device)
+        ptr = lambda t_: t_.data_ptr() if t_ is not None else None  # noqa: E731
+        L_.check(self._lib.mlb_stereo_filter_images(ptr(raw), ptr(dec), ptr(xyzc), C.byref(ib), n_left, n_right,
+                                                    raw.shape[1], ptr(out['sel_raw']), ptr(out['sel_dec']),
+                                                    ptr(out['sel_xyzc']), out['sel_idx'].data_ptr(),
+                                                    out['n_sel'].data_ptr(), out['sel_img_off'].data_ptr(),
+                                                    cnt.data_ptr(), best.data_ptr(), self._stream()),
+                 'mlb_stereo_filter_images')
+        if not trim:
+            return out
+        n = int(out['n_sel'].item())
+        out['sel_img_off'] = out['sel_img_off'].cpu().tolist()
+        for k in ('sel_raw', 'sel_dec', 'sel_xyzc', 'sel_idx'):
+            if out[k] is not None:
+                out[k] = out[k][:n]
+        return out
+
     def stereo_filter_host(self, raw, dec, xyzc, n_left, n_right):
         """The filter for callers that want HOST tensors (Loco.forward): the count and the first n_left + 8 candidate rows
         travel in one batch of asynchronous copies followed by ONE synchronisation; only when ties push the kept-row
@@ -249,14 +383,23 @@ class LocoEngine:
             return st['raw'][:n].clone(), st['dec'][:n].clone(), st['xyzc'][:n].clone()
         return sel_raw[:n].cpu(), sel_dec[:n].cpu(), sel_xyzc[:n].cpu()
 
-    def epistemic_std(self, x, n_dropout, n_samples=100, seed=1, kind=L_.IN_X, kk=None):
+    def epistemic_std(self, x, n_dropout, n_samples=100, seed=1, kind=L_.IN_X, kk=None, row_off=None, kk_list=None,
+                      zero_center=False):
         """net.py:135-161: n_dropout stochastic forwards (top-level dropout on) -> (d, bi) -> Laplace sampling -> std.
         The passes are independent rows to the kernel: the inputs are replicated n_dropout times and run as ONE
         launch (the dropout mask is a function of (seed, site, row, column), so every replica draws its own mask and
-        the weights are streamed once for all passes instead of once per pass).  Returns a CUDA tensor [B]."""
+        the weights are streamed once for all passes instead of once per pass).  Returns a CUDA tensor [B].
+        Images form (row_off + kk_list, keypoints x of all images, mono; zero_center for the legacy monoloco): the image
+        CSR is tiled n_dropout times on the host and the replicas run as one forward_images launch."""
         B = x.shape[0]
         reps = x.repeat((n_dropout,) + (1,) * (x.dim() - 1))
-        out = self.forward(reps, kk=kk, kind=kind, dropout=True, drop_seed=seed)
+        if row_off is not None:
+            row_off = np.asarray(row_off, dtype=np.int64)
+            tiled = np.concatenate([[0]] + [row_off[1:] + p * B for p in range(n_dropout)])
+            out = self.forward_images(reps, tiled, list(kk_list) * n_dropout, kind=L_.IN_KPS, zero_center=zero_center,
+                                      dropout=True, drop_seed=seed)
+        else:
+            out = self.forward(reps, kk=kk, kind=kind, dropout=True, drop_seed=seed)
         c0 = 0 if self.output_size == 2 else 2  # net.py:146-149: db = outputs[:, 0:2] (monoloco) | outputs[:, 2:4]
         d_bi = torch.stack((out['raw'][:, c0], out['dec'][:, 4]), dim=1).contiguous()  # [n_dropout * B, 2] = [N, B, 2]
         std = torch.empty((B,), dtype=torch.float32, device=self.device)

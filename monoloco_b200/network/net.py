@@ -127,6 +127,93 @@ class Loco:
                 dic_out['epi'] = [0.] * n_out
         return dic_out
 
+    def forward_batch(self, keypoints_list, kk_list, keypoints_r_list=None):
+        """Loco.forward over many images with ONE network launch (plus two for the monstereo filter): image i gets the dict
+        forward(keypoints_list[i], kk_list[i], keypoints_r_list[i]) returns, or None when it has no detections
+        (net.py:88-89).  Inputs are staged through pinned memory, every copy back is asynchronous and the call ends in
+        one stream synchronisation.  MC-dropout epistemic std (mono nets) adds one launch for all images' passes."""
+        import numpy as np
+        from ..engine import image_offsets
+        n_img = len(keypoints_list)
+        if len(kk_list) != n_img:
+            raise ValueError("forward_batch: one camera matrix per image")
+        n_l = [len(k) for k in keypoints_list]
+        res = [None] * n_img
+        if sum(n_l) == 0:
+            return res
+        eng = self.model.engine()
+        stereo = self.net == 'monstereo'
+        with torch.no_grad():
+            kps_h = self._pinned('b_kps', (sum(n_l), 3, 17), torch.float32)
+            kps_h.copy_(torch.from_numpy(np.concatenate([np.asarray(k, dtype=np.float32).reshape(-1, 3, 17)
+                                                         for k in keypoints_list if len(k)])))
+            kps = kps_h.to(self.device, non_blocking=True)
+            if stereo:
+                rights = []
+                for i, k in enumerate(keypoints_list):
+                    kr = keypoints_r_list[i] if keypoints_r_list is not None else None
+                    if not len(k):
+                        rights.append(np.zeros((0, 3, 17), dtype=np.float32))
+                    elif kr is None or not len(kr):
+                        rights.append(np.asarray(k[0:1], dtype=np.float32).reshape(1, 3, 17))  # net.py:115-116
+                    else:
+                        rights.append(np.asarray(kr, dtype=np.float32).reshape(-1, 3, 17))
+                n_r = [r.shape[0] for r in rights]
+                kr_h = self._pinned('b_kps_r', (sum(n_r), 3, 17), torch.float32)
+                kr_h.copy_(torch.from_numpy(np.concatenate(rights)))
+                kps_r = kr_h.to(self.device, non_blocking=True)
+                left_off, right_off = image_offsets(n_l), image_offsets(n_r)
+                row_off = image_offsets([a * b for a, b in zip(n_l, n_r)])
+                out = eng.forward_images(kps, row_off, kk_list, kind=L_.IN_KPS_STEREO, x_right=kps_r, left_off=left_off,
+                                         right_off=right_off, want_xyzc=True)
+                sel = eng.stereo_filter_images(out['raw'], out['dec'], row_off, left_off, right_off, xyzc=out['xyzc'],
+                                               trim=False)  # process.py:307-327 per image
+                dev = {'raw': sel['sel_raw'], 'dec': sel['sel_dec'], 'xyzc': sel['sel_xyzc'], 'off': sel['sel_img_off']}
+            else:
+                row_off = image_offsets(n_l)
+                zc = self.net == 'monoloco'
+                out = eng.forward_images(kps, row_off, kk_list, kind=L_.IN_KPS, want_xyzc=True, zero_center=zc)
+                dev = {'raw': out['raw'], 'dec': out['dec'], 'xyzc': out['xyzc']}
+                if self.n_dropout > 0:
+                    dev['epi'] = eng.epistemic_std(kps, self.n_dropout, n_samples=self.N_SAMPLES, seed=1, row_off=row_off,
+                                                   kk_list=kk_list, zero_center=zc)
+            host = {}
+            for k, v in dev.items():
+                host[k] = self._pinned('b_' + k, tuple(v.shape), v.dtype)
+                host[k].copy_(v, non_blocking=True)
+            torch.cuda.current_stream(self.device).synchronize()
+        eng.check_error()
+        off = host['off'].tolist() if stereo else row_off.tolist()
+        for i in range(n_img):
+            if not n_l[i]:
+                continue
+            a, b = off[i], off[i + 1]
+            raw, dec = host['raw'][a:b].clone(), host['dec'][a:b].clone()
+            if stereo:
+                dic = dec_to_dict(raw, dec, stereo=True)
+            elif self.net == 'monoloco':
+                dic = {'d': raw[:, 0:1], 'bi': dec[:, 4:5]}  # net.py:95-100
+            elif self.net == 'monoloco_p':
+                dic = {'xyz': raw[:, 0:3], 'zb': raw[:, 2:4], 'h': raw[:, 4:5], 'w': raw[:, 5:6], 'l': raw[:, 6:7],
+                       'ori': raw[:, 7:9], 'xyzd': dec[:, 0:4], 'd': dec[:, 3:4], 'bi': dec[:, 4:5],
+                       'yaw': (dec[:, 5:6], dec[:, 6:7])}  # extract_outputs_mono, process.py:330-360
+            else:
+                dic = dec_to_dict(raw, dec, stereo=False)
+            dic['xyz_c'] = host['xyzc'][a:b, 0:3].clone()
+            dic['epi'] = host['epi'][a:b].clone() if 'epi' in host else [0.] * n_l[i]
+            res[i] = dic
+        return res
+
+    def _pinned(self, name, shape, dtype):
+        """Pinned host buffer of this Loco, reused across calls (each call synchronises before it returns)."""
+        import math
+        n = math.prod(shape)
+        st = self.__dict__.setdefault('_pin', {})
+        buf = st.get(name)
+        if buf is None or buf.numel() < n or buf.dtype != dtype:
+            buf = st[name] = torch.empty((max(n, 64),), dtype=dtype).pin_memory()
+        return buf[:n].view(shape)
+
     def _forward_host_mono(self, eng, keypoints, kk):
         """Python lists -> pinned staging -> mlb_forward_host -> fresh CPU tensors (caller owns them, net.py contract)."""
         import numpy as np
