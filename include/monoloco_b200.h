@@ -240,6 +240,38 @@ int mlb_post_process(const mlb_post_args* args, void* stream);
 int mlb_kitti_rows(int n, int out_size, double conf_scale, const double* boxes, const float* raw, const float* dec,
                    const float* epi, double* rows, void* stream);
 
+/* ---- activity heuristics for a BATCH of images (Loco.social_distance / Loco.raising_hand, net.py:250-271;
+ * activity.py:17-67, 70-117, 120-165).  People of all images are concatenated in each image's list order (a person's
+ * position selects its Laplace draw); img_off are CSR offsets.  One CTA per image (grid-stride), the image's people
+ * staged in shared memory, one warp per (person, neighbour) pair with lanes over the samples.  The flags equal the
+ * reference's bit for bit: fp64 in the reference's operation order, fp32 where it computes on torch tensors, and the
+ * draws dds[p] - |stds[p]| * table[s * n + p] of the seed-1 stream (n = people in the image). */
+#define MLB_SOCIAL_MAX_PEOPLE 1024  /* largest image (shared-memory layout); crowds in KITTI / Collective Activity are < 100 */
+#define MLB_SOCIAL_MAX_RADII 8
+typedef struct mlb_social_args {
+    int32_t n_img;             /* >= 1                                                                               */
+    int32_t n_people;          /* rows of xz / angles / dds / stds / out over all images                            */
+    int32_t max_people;        /* largest image, 0..MLB_SOCIAL_MAX_PEOPLE (shared-memory sizing; images are clamped)  */
+    int32_t n_samples;         /* Laplace samples per person; < 2 selects the deterministic test (activity.py:34-39) */
+    int32_t n_radii;           /* 1..MLB_SOCIAL_MAX_RADII                                                            */
+    int32_t social_distance;   /* halve the o-space gap (activity.py:148-149)                                        */
+    int64_t table_len;         /* entries of `table`; >= n_samples * max_people when n_samples >= 2                  */
+    double threshold_prob;     /* share of draws in which the F-formation must hold                                 */
+    double threshold_dist;     /* neighbours farther than this (m) are not tested                                   */
+    double radii[MLB_SOCIAL_MAX_RADII];
+    const int32_t* img_off;    /* [n_img + 1] device                                                                 */
+    const double* xz;          /* [n_people][2] device, centre (x, z)                                                */
+    const double* angles;      /* [n_people] device, orientation (rad)                                               */
+    const float* dds;          /* [n_people] device, distance (unused when n_samples < 2)                            */
+    const float* stds;         /* [n_people] device, Laplace scale, sign ignored (unused when n_samples < 2)         */
+    const float* table;        /* [table_len] device, sign(u) * log1p(-|u|) of torch's seed-1 uniform_(eps - 1, 1)   */
+    uint8_t* out;              /* [n_people] device, 1 = interacting                                                 */
+} mlb_social_args;
+/* Asynchronous on `stream`, one launch; rejects bad arguments with mlb_last_error() before launching. */
+int mlb_social_distance(const mlb_social_args* args, void* stream);
+/* is_raising_hand for n poses kps [n][3][17] fp64 (device): out[i] = 0 none, 1 left, 2 right, 3 both. */
+int mlb_raising_hand(const double* kps, int n, int8_t* out, void* stream);
+
 /* decode only (process.py:231-278 / 330-360 on a raw tensor that did not come from mlb_forward):
  * raw [B, out_size] -> dec [B, 8] as in mlb_forward_args.out_dec.  Device buffers. */
 int mlb_decode(const float* raw, int n_rows, int out_size, int decode_kind, float* dec, void* stream);

@@ -24,7 +24,7 @@ KERNEL_NAMES = {0: 'loco_forward_kernel (FFMA row tiles)', 1: 'loco_forward_clus
                 4: 'loco_forward_wide2_kernel (FFMA, 4-CTA clusters, K x N split)'}
 
 EXPORTS = ['mlb_create', 'mlb_update_weights', 'mlb_destroy', 'mlb_last_error', 'mlb_abi_version', 'mlb_num_sms', 'mlb_device_error', 'mlb_last_kernel', 'mlb_tc_resident_clusters', 'mlb_kernel_times',
-           'mlb_forward', 'mlb_forward_host', 'mlb_forward_images', 'mlb_preprocess', 'mlb_stereo_filter', 'mlb_stereo_filter_images', 'mlb_post_process', 'mlb_kitti_rows', 'mlb_decode', 'mlb_laplace_std', 'mlb_ipc_alloc', 'mlb_ipc_open', 'mlb_ipc_close', 'mlb_ipc_free', 'mlb_train_create', 'mlb_train_destroy',
+           'mlb_forward', 'mlb_forward_host', 'mlb_forward_images', 'mlb_preprocess', 'mlb_stereo_filter', 'mlb_stereo_filter_images', 'mlb_post_process', 'mlb_kitti_rows', 'mlb_social_distance', 'mlb_raising_hand', 'mlb_decode', 'mlb_laplace_std', 'mlb_ipc_alloc', 'mlb_ipc_open', 'mlb_ipc_close', 'mlb_ipc_free', 'mlb_train_create', 'mlb_train_destroy',
            'mlb_train_forward', 'mlb_train_backward', 'mlb_train_step', 'mlb_train_phase_times', 'mlb_train_subphase_times',
            'mlb_adam_clip_step',
            'mlb_probe_ffma',
@@ -64,6 +64,18 @@ class MlbPostArgs(C.Structure):
                 ('kps', C.c_void_p), ('kinv', C.c_void_p), ('dec', C.c_void_p), ('gt_boxes', C.c_void_p),
                 ('gt_d', C.c_void_p), ('xyz', C.c_void_p), ('ray', C.c_void_p), ('conf', C.c_void_p), ('uv', C.c_void_p),
                 ('match_gt', C.c_void_p), ('order', C.c_void_p), ('n_match', C.c_void_p), ('xyz_real', C.c_void_p)]
+
+
+SOCIAL_MAX_PEOPLE = 1024
+SOCIAL_MAX_RADII = 8
+
+
+class MlbSocialArgs(C.Structure):
+    _fields_ = [('n_img', C.c_int32), ('n_people', C.c_int32), ('max_people', C.c_int32), ('n_samples', C.c_int32),
+                ('n_radii', C.c_int32), ('social_distance', C.c_int32), ('table_len', C.c_int64),
+                ('threshold_prob', C.c_double), ('threshold_dist', C.c_double), ('radii', C.c_double * SOCIAL_MAX_RADII),
+                ('img_off', C.c_void_p), ('xz', C.c_void_p), ('angles', C.c_void_p), ('dds', C.c_void_p),
+                ('stds', C.c_void_p), ('table', C.c_void_p), ('out', C.c_void_p)]
 
 
 MLB_MAX_BLOCKS = 16
@@ -126,6 +138,8 @@ def lib():
     l.mlb_post_process.argtypes = [C.POINTER(MlbPostArgs), C.c_void_p]
     l.mlb_kitti_rows.argtypes = [C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]
+    l.mlb_social_distance.argtypes = [C.POINTER(MlbSocialArgs), C.c_void_p]
+    l.mlb_raising_hand.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     l.mlb_decode.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     l.mlb_laplace_std.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p]
     l.mlb_ipc_alloc.argtypes = [C.c_int, C.c_size_t, C.POINTER(C.c_void_p), C.c_char_p]

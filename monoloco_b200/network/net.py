@@ -310,3 +310,96 @@ class Loco:
         """net.py:267-271."""
         dic_out['raising_hand'] = [is_raising_hand(keypoint) for keypoint in keypoints]
         return dic_out
+
+    @staticmethod
+    def social_distance_batch(dic_out_list, args):
+        """Loco.social_distance over many images in ONE launch (social_distance_device): every dictionary gets the
+        'social_distance' list the per-image method writes, flag for flag (same args.threshold_prob / threshold_dist /
+        radii, social_distance=False, 100 samples).  An empty dictionary gets [], and a None entry becomes an empty
+        defaultdict(list) with [] (what post_process gives an image without detections).  Inputs go through pinned
+        memory and the call ends in one stream synchronisation.  Raises ValueError where the reference's Laplace
+        constructor would, before anything is launched.  Returns the list of dictionaries."""
+        import numpy as np
+        from .post import social_distance_device, check_laplace_args
+        res = [defaultdict(list) if d is None else d for d in dic_out_list]
+        for d in res:
+            if isinstance(d, defaultdict):   # the per-image method's reads create these keys on post_process's dicts
+                d['angles'], d['dds_pred'], d['stds_ale'], d['xyz_pred']  # noqa: B018
+        counts = [len(d['xyz_pred']) if 'xyz_pred' in d else 0 for d in res]
+        n = sum(counts)
+        if n == 0:
+            for d in res:
+                d['social_distance'] = []
+            return res
+        live = [d for d, c in zip(res, counts) if c]
+        xz = np.concatenate([np.asarray(d['xyz_pred'], dtype=np.float64).reshape(-1, 3)[:, (0, 2)] for d in live])
+        ang = np.concatenate([np.asarray(d['angles'], dtype=np.float64).reshape(-1) for d in live])
+        dds = np.concatenate([np.asarray(d['dds_pred'], dtype=np.float32).reshape(-1) for d in live])
+        stds = np.concatenate([np.asarray(d['stds_ale'], dtype=np.float32).reshape(-1) for d in live])
+        if not (len(ang) == len(dds) == len(stds) == n):
+            raise ValueError("social_distance_batch: angles, dds_pred and stds_ale need one entry per person")
+        check_laplace_args(dds, stds)   # laplace_sampling (process.py:101-122) with the default 100 samples
+        dev = torch.device('cuda', torch.cuda.current_device())
+        h64, h32 = _pinned_host('sd64', (3 * n,), torch.float64), _pinned_host('sd32', (2 * n,), torch.float32)
+        h64[:2 * n].copy_(torch.from_numpy(xz.reshape(-1)))
+        h64[2 * n:].copy_(torch.from_numpy(ang))
+        h32[:n].copy_(torch.from_numpy(dds))
+        h32[n:].copy_(torch.from_numpy(stds))
+        d64, d32 = h64.to(dev, non_blocking=True), h32.to(dev, non_blocking=True)
+        flags = social_distance_device(d64[:2 * n].view(n, 2), d64[2 * n:], d32[:n], d32[n:], np.cumsum([0] + counts),
+                                       threshold_prob=args.threshold_prob, threshold_dist=args.threshold_dist,
+                                       radii=args.radii, n_samples=Loco.N_SAMPLES)
+        h_out = _pinned_host('sd_out', (n,), torch.bool)
+        h_out.copy_(flags, non_blocking=True)
+        torch.cuda.current_stream(dev).synchronize()
+        vals = h_out.tolist()
+        pos = 0
+        for d, c in zip(res, counts):
+            d['social_distance'] = vals[pos:pos + c]
+            pos += c
+        return res
+
+    @staticmethod
+    def raising_hand_batch(dic_out_list, keypoints_list):
+        """Loco.raising_hand over many images in ONE launch (raising_hand_device): dictionary i gets
+        [is_raising_hand(k) for k in keypoints_list[i]], in the caller's keypoint order as net.py:269-271 does.  None
+        entries become an empty defaultdict(list).  Pinned staging, one stream synchronisation.  Returns the list."""
+        import numpy as np
+        from .post import raising_hand_device, RAISING_HAND
+        if len(keypoints_list) != len(dic_out_list):
+            raise ValueError("raising_hand_batch: one keypoint list per dictionary")
+        res = [defaultdict(list) if d is None else d for d in dic_out_list]
+        counts = [len(k) if k is not None else 0 for k in keypoints_list]
+        n = sum(counts)
+        if n == 0:
+            for d in res:
+                d['raising_hand'] = []
+            return res
+        kps = np.concatenate([np.asarray(k, dtype=np.float64).reshape(-1, 3, 17) for k, c in zip(keypoints_list, counts) if c])
+        dev = torch.device('cuda', torch.cuda.current_device())
+        h_kps = _pinned_host('rh_kps', (n, 3, 17), torch.float64)
+        h_kps.copy_(torch.from_numpy(kps))
+        codes = raising_hand_device(h_kps.to(dev, non_blocking=True))
+        h_out = _pinned_host('rh_out', (n,), torch.int8)
+        h_out.copy_(codes, non_blocking=True)
+        torch.cuda.current_stream(dev).synchronize()
+        vals = [RAISING_HAND[c] for c in h_out.tolist()]
+        pos = 0
+        for d, c in zip(res, counts):
+            d['raising_hand'] = vals[pos:pos + c]
+            pos += c
+        return res
+
+
+_PINNED = {}
+
+
+def _pinned_host(name, shape, dtype):
+    """Pinned host buffer shared by the static batch methods, reused across calls (each call synchronises before it
+    returns)."""
+    import math
+    n = math.prod(shape)
+    buf = _PINNED.get(name)
+    if buf is None or buf.numel() < n or buf.dtype != dtype:
+        buf = _PINNED[name] = torch.empty((max(n, 64),), dtype=dtype).pin_memory()
+    return buf[:n].view(shape)

@@ -142,3 +142,104 @@ def kitti_rows_device(boxes, raw, dec, epi=None, net='monoloco_pp'):
                                 raw.data_ptr(), dec.data_ptr(), d_epi.data_ptr() if d_epi is not None else None,
                                 rows.data_ptr(), _stream(dev)), 'mlb_kitti_rows')
     return rows.cpu().numpy()
+
+
+# ------------------------------------------------------------------------------------------------ activity heuristics
+_DRAW_TABLES = {}   # torch.device -> CUDA fp32 draw table (laplace_draw_table), grown on demand
+
+
+def laplace_draw_table(n):
+    """The draws behind the reference's social-distancing samples, as a table: T[k] = sign(u_k) * log1p(-|u_k|) for the
+    first n values u of torch's seed-1 CPU stream `uniform_(eps - 1, 1)` (fp32).  laplace_sampling (process.py:101-122)
+    reseeds with torch.manual_seed(1) on every call, so for an image of n people the S x n draws are
+    dds[p] - |stds[p]| * T[s * n + p], bit for bit (Laplace.rsample computes loc - scale * u.sign() * log1p(-|u|)).  The
+    stream is a prefix stream, so a longer table starts with every shorter one.  A private generator is used: the global
+    CPU generator is left untouched.  torch computes log1p here because a device log1pf rounds differently."""
+    g = torch.Generator().manual_seed(1)
+    u = torch.empty(int(n), dtype=torch.float32).uniform_(torch.finfo(torch.float32).eps - 1, 1, generator=g)
+    return u.sign() * torch.log1p(-u.abs())
+
+
+def _draw_table(n, dev):
+    t = _DRAW_TABLES.get(dev)
+    if t is None or t.numel() < n:
+        size = max(int(n), 6400, 2 * (t.numel() if t is not None else 0))
+        t = _DRAW_TABLES[dev] = laplace_draw_table(size).to(dev)
+    return t
+
+
+def check_laplace_args(dds, stds):
+    """Raise ValueError where the reference's torch.distributions.Laplace(dds, |stds|) would (fp32 values): a NaN
+    distance or a scale that is not > 0 (zero, NaN, or too small for fp32)."""
+    d = np.asarray(dds, dtype=np.float32).reshape(-1)
+    s = np.abs(np.asarray(stds, dtype=np.float32).reshape(-1))
+    if np.isnan(d).any():
+        raise ValueError("social distance: a distance is NaN (Laplace loc must be real)")
+    if not (s > 0).all():
+        raise ValueError("social distance: a std is zero or NaN in fp32 (Laplace scale must be positive)")
+
+
+def social_distance_device(xz, angles, dds, stds, img_off, *, threshold_prob, threshold_dist, radii, social_distance=False,
+                           n_samples=100, max_people=None):
+    """`social_interactions(idx, ...)` (activity.py:17-67) for every person of every image, in one launch
+    (mlb_social_distance), flags identical to the reference's.  Device tensors in, a CUDA bool tensor [n] out, no host
+    synchronisation.
+      xz [n, 2] centres (x, z), angles [n] (fp64 on the device; other float dtypes are converted), dds [n], stds [n]
+      (fp32, as torch.tensor(dds) makes them); people of all images concatenated, each image in its list order (the
+      position selects the draw).  After LocoEngine.forward_images: xyzc[:, (0, 2)], dec[:, 5], dec[:, 3], dec[:, 4].
+      img_off: CSR offsets [n_img + 1].  Host offsets (sequence, numpy, CPU tensor) are checked here and give the largest
+      image; CUDA offsets need `max_people`, and the kernel clamps every image to it.
+    The reference's validity check of Laplace(dds, stds) is not repeated here (it needs the values on the host):
+    Loco.social_distance_batch does it."""
+    lib = L_.lib()
+    if not xz.is_cuda:
+        raise ValueError("social_distance_device: inputs must be CUDA tensors")
+    dev = xz.device
+    n = xz.shape[0]
+    if isinstance(img_off, torch.Tensor) and img_off.is_cuda:
+        if max_people is None:
+            raise ValueError("social_distance_device: max_people is required with device offsets")
+        d_off = img_off.to(torch.int32).contiguous()
+    else:
+        off = np.asarray(img_off.cpu() if isinstance(img_off, torch.Tensor) else img_off, dtype=np.int64).reshape(-1)
+        if off.size < 2 or off[0] != 0 or off[-1] != n or (np.diff(off) < 0).any():
+            raise ValueError("social_distance_device: img_off must rise from 0 to %d" % n)
+        if max_people is None:
+            max_people = int(np.diff(off).max())
+        d_off = torch.from_numpy(off.astype(np.int32)).to(dev, non_blocking=True)
+    out = torch.empty((n,), dtype=torch.uint8, device=dev)
+    radii = [float(r) for r in radii]
+    a = L_.MlbSocialArgs()
+    a.n_img, a.n_people, a.max_people, a.n_samples = d_off.numel() - 1, n, int(max_people), int(n_samples)
+    a.n_radii, a.social_distance = len(radii), int(bool(social_distance))
+    a.threshold_prob, a.threshold_dist = float(threshold_prob), float(threshold_dist)
+    for i, r in enumerate(radii[:L_.SOCIAL_MAX_RADII]):
+        a.radii[i] = r
+    xz64 = xz.to(torch.float64).contiguous()
+    ang64 = angles.to(torch.float64).contiguous()
+    keep = [xz64, ang64]
+    if n_samples >= 2:
+        table = _draw_table(max(int(n_samples), 0) * min(max(int(max_people), 0), L_.SOCIAL_MAX_PEOPLE), dev)
+        d32, s32 = dds.to(torch.float32).contiguous(), stds.to(torch.float32).contiguous()
+        keep += [d32, s32]
+        a.dds, a.stds, a.table, a.table_len = d32.data_ptr(), s32.data_ptr(), table.data_ptr(), table.numel()
+    a.img_off, a.xz, a.angles, a.out = d_off.data_ptr(), xz64.data_ptr(), ang64.data_ptr(), out.data_ptr()
+    L_.check(lib.mlb_social_distance(C.byref(a), _stream(dev)), 'mlb_social_distance')
+    return out.view(torch.bool)
+
+
+RAISING_HAND = (None, 'left', 'right', 'both')   # codes of mlb_raising_hand
+
+
+def raising_hand_device(kps):
+    """`is_raising_hand` (activity.py:70-117) for every pose: CUDA kps [n, 3, 17] (fp64 on the device) -> CUDA int8 codes
+    [n] (0 None, 1 left, 2 right, 3 both; RAISING_HAND maps them back), one launch, no host synchronisation."""
+    if not kps.is_cuda:
+        raise ValueError("raising_hand_device: kps must be a CUDA tensor")
+    k64 = kps.to(torch.float64).contiguous()
+    n = k64.shape[0]
+    if n and tuple(k64.shape[1:]) != (3, 17):
+        raise ValueError("raising_hand_device: kps must be [n, 3, 17]")
+    out = torch.empty((n,), dtype=torch.int8, device=kps.device)
+    L_.check(L_.lib().mlb_raising_hand(k64.data_ptr(), n, out.data_ptr(), _stream(kps.device)), 'mlb_raising_hand')
+    return out

@@ -169,3 +169,25 @@ def make_kitti_case(net, n=7, seed=0):
         first = [[float(v) for v in row] for row in xyz] if net == 'baseline' else f32(d)
         outs = [first, f32(bi), f32(epi), zzs, centers]
     return boxes, outs, [kk, tt], cat
+
+
+def make_crowd(n, seed=0, spacing=(0.3, 3.0)):
+    """One image's people for the activity heuristics (Loco.social_distance inputs): n centres (x, z) in metres, each
+    new one `spacing` m from an earlier one and at least spacing[0] from all, orientations in (-pi, pi], distances
+    near |centre| and Laplace scales in [0.2, 1].  Python lists of floats, as post_process writes them."""
+    rng = np.random.RandomState(seed)
+    pts = []
+    while len(pts) < n:
+        if not pts:
+            c = (rng.uniform(-3.0, 3.0), rng.uniform(4.0, 12.0))
+        else:
+            base = pts[rng.randint(len(pts))]
+            r, a = rng.uniform(*spacing), rng.uniform(-math.pi, math.pi)
+            c = (base[0] + r * math.cos(a), base[1] + r * math.sin(a))
+        if all(math.hypot(c[0] - p[0], c[1] - p[1]) >= spacing[0] for p in pts):
+            pts.append(c)
+    centers = [[float(x), float(z)] for x, z in pts]
+    angles = rng.uniform(-math.pi, math.pi, n).tolist()
+    dds = [math.hypot(x, z) * float(rng.uniform(0.95, 1.05)) for x, z in centers]
+    stds = rng.uniform(0.2, 1.0, n).tolist()
+    return centers, angles, dds, stds
