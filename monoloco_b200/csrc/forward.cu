@@ -953,7 +953,9 @@ static int forward_impl(mlb_handle h, const mlb_forward_args* a, const ImgParams
 
     // ---- large batches (and every batch of a model wider than the FFMA kernels cover): error-compensated TF32 on the
     // tensor cores, persistent CTA groups over 64-row tiles (forward_tc.cu)
-    const bool forced_ffma = (a->flags & (MLB_FWD_FORCE_TILE | MLB_FWD_FORCE_CLUSTER | MLB_FWD_FORCE_WIDE)) != 0 || a->rows_per_group != 0;
+    // A forced FFMA kernel (wide2 included) either runs or is refused: it never falls through to the tensor cores.
+    const bool forced_ffma = (a->flags & (MLB_FWD_FORCE_TILE | MLB_FWD_FORCE_CLUSTER | MLB_FWD_FORCE_WIDE | MLB_FWD_FORCE_WIDE2)) != 0 ||
+                             a->rows_per_group != 0;
     if ((a->flags & MLB_FWD_FORCE_TC) && h->tc == nullptr)
         return fail("mlb_forward: the tensor-core kernel is not available for this model (linear_size % 256 != 0)");
     if (!h->ffma_ok && forced_ffma) return fail("mlb_forward: this model width runs on the tensor-core kernel only");
