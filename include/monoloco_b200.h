@@ -287,7 +287,8 @@ int mlb_laplace_std(const float* d_bi, int n_pass, int n_rows, int n_samples, ui
  * grid-wide reduction per layer, Dropout with a counter RNG or explicit masks, running-stat update) and backward
  * (dL/dout -> every parameter gradient); mlb_train_step fuses forward + MultiTaskLoss + backward in ONE launch.
  * All pointers are device pointers to fp32 tensors in the reference's native layouts (nn.Linear.weight [out,in]).
- * LocoModel topology only (architectures.py:48-71), which is what Trainer builds (trainer.py:115-122). */
+ * Topologies: LocoModel (architectures.py:48-71, what Trainer builds, trainer.py:115-122) with its aux head, and
+ * MonolocoModel (architectures.py:135-176) with aux_block = -1; mlb_train_step (the fused loss) needs LocoModel. */
 #define MLB_MAX_BLOCKS 16
 enum { MLB_TASK_D = 0, MLB_TASK_X = 1, MLB_TASK_Y = 2, MLB_TASK_H = 3, MLB_TASK_W = 4, MLB_TASK_L = 5,
        MLB_TASK_ORI = 6, MLB_TASK_AUX = 7 };  /* trainer.py:40, losses.py:76-101 */
@@ -295,7 +296,7 @@ enum { MLB_TASK_D = 0, MLB_TASK_X = 1, MLB_TASK_Y = 2, MLB_TASK_H = 3, MLB_TASK_
 typedef struct mlb_train_block {   /* one L-wide Linear (+BatchNorm1d+ReLU+Dropout) in forward order; every    */
                                    /* shape is the caller's real one (L = linear_size, padding is internal)    */
     int32_t K;                     /* in_features: input_size for block 0, linear_size for the others          */
-    int32_t has_bn;                /* 0 only for LocoModel.w2 (architectures.py:59)                            */
+    int32_t has_bn;                /* 0 only for LocoModel.w2 (architectures.py:59); 1 everywhere in MonolocoModel */
     int32_t res_src;               /* index of the block whose output is added to this one's (x + y), or -1   */
     int32_t reserved;
     const float* W;                /* [L, K]                                                                   */
@@ -313,6 +314,9 @@ typedef struct mlb_train_block {   /* one L-wide Linear (+BatchNorm1d+ReLU+Dropo
 typedef struct mlb_train_args {
     int32_t n_rows, input_size, output_size, linear_size, n_blocks;
     int32_t aux_block;             /* block whose output feeds w_aux (LocoModel.w2); w_fin reads the last block */
+                                   /* -1: no aux head (MonolocoModel): output_size = w_fin rows in [1,16],       */
+                                   /* W_aux/b_aux/dW_aux/db_aux may be NULL, every block has BatchNorm, the last */
+                                   /* block may carry a residual; mlb_train_step rejects it                      */
     int32_t update_running_stats;  /* 1 in training (nn.BatchNorm1d momentum update, unbiased variance)         */
     int32_t rows_per_group;        /* 0 = auto                                                                  */
     float p_dropout, bn_eps, bn_momentum;
@@ -320,7 +324,7 @@ typedef struct mlb_train_args {
     uint64_t drop_seed;            /* counter-RNG seed (must be the same in forward and backward)               */
     const uint8_t* drop_mask;      /* optional explicit keep masks [n_bn_blocks][B][L], L = linear_size         */
     const float* x;                /* [B, input_size] pre-processed inputs                                      */
-    float* out;                    /* [B, output_size]                                                          */
+    float* out;                    /* [B, output_size]: [w_fin | w_aux], or w_fin alone with aux_block = -1     */
     const float* g_out;            /* backward only: dL/d(out) [B, output_size]                                 */
     const float* W_aux; const float* b_aux; const float* W_fin; const float* b_fin;   /* [1,L],[1],[out-1,L],[out-1] */
     float* dW_aux; float* db_aux; float* dW_fin; float* db_fin;

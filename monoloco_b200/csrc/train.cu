@@ -4,6 +4,7 @@
 // Replaces (reference file:line):
 //   monoloco/train/trainer.py:153-161      outputs = model(inputs); loss, _ = mt_loss(outputs, labels); loss.backward()
 //   monoloco/network/architectures.py:48-71, 88-102   LocoModel / MyLinearSimple forward in train mode
+//   monoloco/network/architectures.py:135-176         MonolocoModel / MyLinear forward in train mode
 //                                          (nn.BatchNorm1d batch statistics + running-stat update, nn.Dropout)
 //   monoloco/train/losses.py:46-73, 28-43  MultiTaskLoss / AutoTuneMultiTaskLoss.forward
 //   monoloco/train/losses.py:104-142       LaplacianLoss;  nn.L1Loss, nn.BCEWithLogitsLoss (losses.py:81-83)
@@ -21,13 +22,18 @@
 //                        dL/d(previous activation) (+ residual / aux-head terms) -> sums for the previous BN
 //   DW                   dW_i = Gz_i^T A_i as 32-row x 1024-col tiles streamed over the batch dimension
 //
+// Topologies.  LocoModel: w1, the stages, the BatchNorm-free w2 (aux_block, read by the w_aux head), w3; out = [w_fin | w_aux].
+// MonolocoModel (architectures.py:135-176): w1 and the stages only, aux_block = -1 (no aux head, out = w_fin rows) and
+// the last block carries the residual of its stage, so the head reads the sum x + y that the FWD_FINAL prologue writes.
+// It runs the AUX = false instantiations (loco_train_kernel<TM, EXT, false>); LocoModel's (AUX = true) are unchanged.
+//
 // Widths.  The kernel runs at the padded width L of the forward (packing.py::padded_width): the next multiple of 128
 // up to 1024, of 256 above.  When the caller's width Lr is smaller, PAD copies every parameter (and the explicit
 // dropout masks) into zero-padded workspace tensors first and UNPAD copies the gradients and running statistics back
 // in the caller's shapes last.  A padded unit has zero weights and bias, so Z = 0, its batch mean and variance are 0,
 // zhat = 0 and with beta = 0 its output is exactly 0; dL/dA of it is a sum over zero weight columns, so nothing flows
 // back into the real units.
-// Padded widths and L > 1024 run the EXT instantiations (loco_train_kernel<TM, true>, producer train_producer_ext); the
+// Padded widths and L > 1024 run the EXT instantiations (loco_train_kernel<TM, true, AUX>, producer train_producer_ext); the
 // plain ones (multiples of 128 up to 1024) compile to the same code as before those widths were added.
 // L > 1024 runs every GEMM on two column parts of P = L / 2 <= 1024 columns so that the
 // shared activation tile [P][MP], the weight ring [NSTAGE][KC][P] and the 8-warp x 128-column register tile stay the
@@ -486,6 +492,7 @@ __device__ __forceinline__ void fwd_heads(const TrainParams& p, bool final_phase
 }
 
 // PAD / UNPAD phases (padded widths only): out of line, so that they add no register pressure to the GEMM phases
+template <bool AUX>
 __device__ __noinline__ void pad_phase(const TrainParams& p, int tid, int nfin) {
     const int L = p.L;
     // ---- the caller's Lr-wide tensors -> zero-padded L-wide workspace copies (gamma and running_var pad with 1)
@@ -510,7 +517,8 @@ __device__ __noinline__ void pad_phase(const TrainParams& p, int tid, int nfin) 
             }
         }
     }
-    for (size_t f = g0; f < (size_t)L; f += gs) const_cast<float*>(p.W_aux)[f] = f < (size_t)Lr ? p.uW_aux[f] : 0.f;
+    if constexpr (AUX)
+        for (size_t f = g0; f < (size_t)L; f += gs) const_cast<float*>(p.W_aux)[f] = f < (size_t)Lr ? p.uW_aux[f] : 0.f;
     for (size_t f = g0; f < (size_t)nfin * L; f += gs) {
         const int o = (int)(f / L), k = (int)(f % L);
         const_cast<float*>(p.W_fin)[f] = k < Lr ? p.uW_fin[(size_t)o * Lr + k] : 0.f;
@@ -523,6 +531,7 @@ __device__ __noinline__ void pad_phase(const TrainParams& p, int tid, int nfin) 
         }
 }
 
+template <bool AUX>
 __device__ __noinline__ void unpad_phase(const TrainParams& p, int tid, int nfin) {
     const int L = p.L;
     // ---- gradients (backward) and running statistics (forward) back into the caller's Lr-wide tensors
@@ -544,7 +553,8 @@ __device__ __noinline__ void unpad_phase(const TrainParams& p, int tid, int nfin
             for (size_t f = g0; f < (size_t)Lr; f += gs) u.rmean[f] = b.rmean[f], u.rvar[f] = b.rvar[f];
     }
     if (grads) {
-        for (size_t f = g0; f < (size_t)Lr; f += gs) p.udW_aux[f] = p.dW_aux[f];
+        if constexpr (AUX)
+            for (size_t f = g0; f < (size_t)Lr; f += gs) p.udW_aux[f] = p.dW_aux[f];
         for (size_t f = g0; f < (size_t)nfin * Lr; f += gs) p.udW_fin[f] = p.dW_fin[(f / Lr) * L + f % Lr];
     }
 }
@@ -566,7 +576,9 @@ __device__ __forceinline__ void load_act(float* act, const float* __restrict__ s
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
-template <int TM, bool EXT>
+// AUX: LocoModel's w_aux head is present (aux_block >= 0).  The aux-less MonolocoModel runs the AUX = false
+// instantiations, so that the LocoModel ones compile to the same code as before MonolocoModel was added.
+template <int TM, bool EXT, bool AUX>
 __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid_constant__ TrainParams p) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -615,7 +627,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
     unsigned bar_target = 0;
     const float inv_keep = p.p_drop > 0.f ? 1.0f / (1.0f - p.p_drop) : 1.0f;
     const float invB = 1.0f / (float)p.n_rows;
-    const int nfin = p.out_size - 1;
+    const int nfin = AUX ? p.out_size - 1 : p.out_size;  // rows of the final head
     const uint32_t seed_mix = drop_seed_mix(p.seed), drop_thr = drop_threshold(p.p_drop);
     auto col_hashes = [&](int site, uint32_t (&ch)[8]) {
 #pragma unroll
@@ -679,9 +691,10 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
                 for (int f = blockIdx.x * NT + tid; f < L * L / 4; f += gridDim.x * NT) dw4[f] = make_float4(0.f, 0.f, 0.f, 0.f);
             }
             for (int f = blockIdx.x * NT + tid; f < L * nfin; f += gridDim.x * NT) p.dW_fin[f] = 0.f;
-            for (int f = blockIdx.x * NT + tid; f < L; f += gridDim.x * NT) p.dW_aux[f] = 0.f;
+            if constexpr (AUX)
+                for (int f = blockIdx.x * NT + tid; f < L; f += gridDim.x * NT) p.dW_aux[f] = 0.f;
             if (blockIdx.x == 0 && tid < nfin) p.db_fin[tid] = 0.f;
-            if (blockIdx.x == 0 && tid == 0) p.db_aux[0] = 0.f;
+            if (AUX && blockIdx.x == 0 && tid == 0) p.db_aux[0] = 0.f;
         } else if (type == PH_FWD || type == PH_FWD_FINAL) {
             // ============================================================================ forward
             const bool final_phase = type == PH_FWD_FINAL;
@@ -888,8 +901,10 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
             }
         } else if (type == PH_BWD_HEAD) {
             // ============================================================================ head backward
+            // lb.Aout is what w_fin reads: after MonolocoModel's last stage it already holds the residual sum x + y, and
+            // lb.G = dL/d(that sum) reaches the residual source through its skip_to path in BWD
             const TBlk& lb = p.blk[p.n_blocks - 1];
-            const TBlk& ab = p.blk[p.aux_block];
+            const TBlk& ab = p.blk[AUX ? p.aux_block : p.n_blocks - 1];  // read only with AUX
             const float* gsrc = p.labels != nullptr ? p.g_out : p.g_out_in;
             const int gld = p.labels != nullptr ? OUT_LD : p.out_size;
             build_ptab(p, lb, ptab, tid, false, false);
@@ -931,7 +946,10 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
 #pragma unroll
                         for (int q = 0; q < KQ; ++q) {
                             const size_t off = gr * L + (kq[q] >= 0 ? kq[q] : 0);
-                            a9[q] = lb.Aout[off], a8[q] = ab.Aout[off], zz[q] = lb.Z[off];
+                            if constexpr (AUX)
+                                a9[q] = lb.Aout[off], a8[q] = ab.Aout[off], zz[q] = lb.Z[off];
+                            else
+                                a9[q] = lb.Aout[off], zz[q] = lb.Z[off];
                         }
 #pragma unroll
                         for (int q = 0; q < KQ; ++q) {
@@ -944,7 +962,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
                                     accf[q][o] = fmaf(go[o], a9[q], accf[q][o]);
                                 }
                             }
-                            acca[q] = fmaf(go[nfin], a8[q], acca[q]);
+                            if constexpr (AUX) acca[q] = fmaf(go[nfin], a8[q], acca[q]);
                             lb.G[gr * L + kq[q]] = G;
                             const float zh = (zz[q] - tq[q].x) * tq[q].y;
                             const float y = fmaf(zh, tq[q].z, tq[q].w);
@@ -958,7 +976,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
                     for (int q = 0; q < KQ; ++q) {
                         if (kq[q] < 0) continue;
                         for (int o = 0; o < nfin; ++o) atomicAdd(p.dW_fin + (size_t)o * L + kq[q], accf[q][o]);
-                        atomicAdd(p.dW_aux + kq[q], acca[q]);
+                        if constexpr (AUX) atomicAdd(p.dW_aux + kq[q], acca[q]);
                         atomicAdd(&lb.stat[2 * L + kq[q]], (double)s3[q]);
                         atomicAdd(&lb.stat[3 * L + kq[q]], (double)s4[q]);
                     }
@@ -966,7 +984,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
                 csync();
             }
             if (tid < nfin) atomicAdd(p.db_fin + tid, dbacc);
-            if (tid == nfin) atomicAdd(p.db_aux, dbacc);
+            if (AUX && tid == nfin) atomicAdd(p.db_aux, dbacc);
         } else if (type == PH_BWD) {
             // ============================================================================ backward of block bi
             const TBlk& b = p.blk[bi];
@@ -1065,7 +1083,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
 #pragma unroll
                             for (int j = 0; j < 8; ++j) {
                                 const int col = col_of(n0, j);
-                                wa[j] = (cur - 1 == p.aux_block) ? __ldg(p.W_aux + col) : 0.f;
+                                wa[j] = (AUX && cur - 1 == p.aux_block) ? __ldg(p.W_aux + col) : 0.f;
                                 if (pb.has_bn) {
                                     const double m = pb.stat[col] * (double)invB;
                                     double var = pb.stat[L + col] * (double)invB - m * m;
@@ -1098,7 +1116,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
                                         G[0] += k0.x, G[1] += k0.y, G[2] += k0.z, G[3] += k0.w;
                                         G[4] += k1.x, G[5] += k1.y, G[6] += k1.z, G[7] += k1.w;
                                     }
-                                    if (cur - 1 == p.aux_block) {
+                                    if (AUX && cur - 1 == p.aux_block) {
                                         const float ga = gsr[gr * gld + nfin];
 #pragma unroll
                                         for (int j = 0; j < 8; ++j) G[j] = fmaf(ga, wa[j], G[j]);
@@ -1185,7 +1203,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
 #pragma unroll
                             for (int j = 0; j < 8; ++j) {
                                 const int col = col_of(nc, j);
-                                wa[j] = (cur - 1 == p.aux_block) ? __ldg(p.W_aux + col) : 0.f;
+                                wa[j] = (AUX && cur - 1 == p.aux_block) ? __ldg(p.W_aux + col) : 0.f;
                                 if (pb.has_bn) {
                                     const double m = pb.stat[col] * (double)invB;
                                     double var = pb.stat[L + col] * (double)invB - m * m;
@@ -1218,7 +1236,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
                                         G[0] += k0.x, G[1] += k0.y, G[2] += k0.z, G[3] += k0.w;
                                         G[4] += k1.x, G[5] += k1.y, G[6] += k1.z, G[7] += k1.w;
                                     }
-                                    if (cur - 1 == p.aux_block) {
+                                    if (AUX && cur - 1 == p.aux_block) {
                                         const float ga = gsr[gr * gld + nfin];
 #pragma unroll
                                         for (int j = 0; j < 8; ++j) G[j] = fmaf(ga, wa[j], G[j]);
@@ -1338,9 +1356,9 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) loco_train_kernel(const __grid
                 u += c1 - c0;
             }
         } else if (EXT && type == PH_PAD) {
-            pad_phase(p, tid, nfin);
+            pad_phase<AUX>(p, tid, nfin);
         } else if (EXT && type == PH_UNPAD) {
-            unpad_phase(p, tid, nfin);
+            unpad_phase<AUX>(p, tid, nfin);
         }
         end_phase(ph);
     }
@@ -1471,17 +1489,21 @@ extern "C" void mlb_train_destroy(mlb_train_handle t) {
     delete t;
 }
 
-template <int TM, bool EXT>
+template <int TM, bool EXT, bool AUX>
 static cudaError_t launch_train(const TrainParams& p, int grid, size_t smem, cudaStream_t st) {
-    cudaError_t e = cudaFuncSetAttribute(loco_train_kernel<TM, EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(loco_train_kernel<TM, EXT, AUX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     void* args[] = {(void*)&p};
-    return cudaLaunchCooperativeKernel((void*)loco_train_kernel<TM, EXT>, dim3(grid), dim3(MAX_THREADS), args, smem, st);
+    return cudaLaunchCooperativeKernel((void*)loco_train_kernel<TM, EXT, AUX>, dim3(grid), dim3(MAX_THREADS), args, smem, st);
+}
+template <int TM, bool AUX>
+static cudaError_t launch_train(const TrainParams& p, int grid, size_t smem, cudaStream_t st) {
+    // EXT: padded widths and widths above 1024; the plain instantiations serve multiples of 128 up to 1024
+    return (p.Lr != p.L || p.L > 1024) ? launch_train<TM, true, AUX>(p, grid, smem, st) : launch_train<TM, false, AUX>(p, grid, smem, st);
 }
 template <int TM>
 static cudaError_t launch_train(const TrainParams& p, int grid, size_t smem, cudaStream_t st) {
-    // EXT: padded widths and widths above 1024; the plain instantiations serve multiples of 128 up to 1024
-    return (p.Lr != p.L || p.L > 1024) ? launch_train<TM, true>(p, grid, smem, st) : launch_train<TM, false>(p, grid, smem, st);
+    return p.aux_block >= 0 ? launch_train<TM, true>(p, grid, smem, st) : launch_train<TM, false>(p, grid, smem, st);
 }
 
 static int pick_tm(int n_rows, int n_ctas) {
@@ -1500,10 +1522,21 @@ static int train_launch(mlb_train_handle t, const mlb_train_args* a, const mlb_t
     if (!t || !a || !blocks) return tfail("mlb_train: null argument");
     if (a->n_rows < 2 || a->n_rows > t->max_rows) return tfail("mlb_train: n_rows must be in [2, max_rows] (BatchNorm needs > 1 row)");
     if (a->linear_size != t->Lr || a->n_blocks != t->n_blocks || a->input_size != t->in_size) return tfail("mlb_train: shape differs from mlb_train_create");
-    if (a->output_size < 2 || a->output_size > OUT_LD) return tfail("mlb_train: bad output_size");
-    if (a->aux_block < 0 || a->aux_block >= a->n_blocks - 1) return tfail("mlb_train: bad aux_block");
-    if (!a->x || !a->out || !a->W_aux || !a->b_aux || !a->W_fin || !a->b_fin) return tfail("mlb_train: missing tensor");
-    if (mode >= 1 && (!a->dW_aux || !a->db_aux || !a->dW_fin || !a->db_fin)) return tfail("mlb_train: missing head gradient buffers");
+    if (a->aux_block >= 0) {  // LocoModel: w_fin rows + the concatenated w_aux column
+        if (a->output_size < 2 || a->output_size > OUT_LD) return tfail("mlb_train: bad output_size");
+        if (a->aux_block >= a->n_blocks - 1) return tfail("mlb_train: bad aux_block");
+        if (!a->x || !a->out || !a->W_aux || !a->b_aux || !a->W_fin || !a->b_fin) return tfail("mlb_train: missing tensor");
+        if (mode >= 1 && (!a->dW_aux || !a->db_aux || !a->dW_fin || !a->db_fin)) return tfail("mlb_train: missing head gradient buffers");
+    } else {  // aux_block = -1 (MonolocoModel): no aux head, output_size = the final head's rows, W_aux & co. may be NULL
+        if (a->aux_block != -1) return tfail("mlb_train: bad aux_block (-1 = no aux head, else a block index)");
+        if (mode == 2)
+            return tfail("mlb_train_step: the fused MultiTaskLoss reads LocoModel's output columns; it needs an aux head "
+                         "(aux_block >= 0)");
+        if (a->output_size < 1 || a->output_size > OUT_LD)
+            return tfail("mlb_train: output_size must be in [1,16] without an aux head (aux_block = -1)");
+        if (!a->x || !a->out || !a->W_fin || !a->b_fin) return tfail("mlb_train: missing tensor");
+        if (mode >= 1 && (!a->dW_fin || !a->db_fin)) return tfail("mlb_train: missing head gradient buffers");
+    }
     if (mode == 1 && !a->g_out) return tfail("mlb_train_backward: g_out required");
     if (mode == 2 && (!a->labels || !a->loss_vals || a->n_tasks < 1 || a->n_tasks > 8)) return tfail("mlb_train_step: labels / loss_vals / tasks required");
     if (a->p_dropout < 0.f || a->p_dropout >= 1.f) return tfail("mlb_train: bad p_dropout");
@@ -1550,7 +1583,10 @@ static int train_launch(mlb_train_handle t, const mlb_train_args* a, const mlb_t
     for (int i = 0; i < a->n_blocks; ++i)
         if (p.blk[i].res_src >= 0) p.blk[p.blk[i].res_src].skip_to = i;
     if (!p.blk[a->n_blocks - 1].has_bn) return tfail("mlb_train: the last block must have BatchNorm (LocoModel.w3)");
-    if (p.blk[a->aux_block].has_bn) return tfail("mlb_train: aux_block must be the BatchNorm-free block (LocoModel.w2)");
+    if (a->aux_block >= 0 && p.blk[a->aux_block].has_bn) return tfail("mlb_train: aux_block must be the BatchNorm-free block (LocoModel.w2)");
+    if (a->aux_block < 0)
+        for (int i = 0; i < a->n_blocks; ++i)
+            if (!p.blk[i].has_bn) return tfail("mlb_train: without an aux head (aux_block = -1) every block must have BatchNorm (MonolocoModel)");
     p.n_blocks = a->n_blocks, p.aux_block = a->aux_block, p.L = t->L, p.Lr = t->Lr, p.in_size = a->input_size;
     p.out_size = a->output_size, p.n_rows = a->n_rows;
     p.n_rows_pad = ((a->n_rows + KC - 1) / KC) * KC;

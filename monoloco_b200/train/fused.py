@@ -1,5 +1,5 @@
 """
-Fused training step for the LocoModel mirror (monoloco_b200/csrc/train.cu).
+Fused training step for the LocoModel and MonolocoModel mirrors (monoloco_b200/csrc/train.cu).
 
 Two ways in, both replacing trainer.py:153-161 (`outputs = model(inputs)`, `mt_loss`, `loss.backward()`):
   * drop-in: `model(inputs)` in train mode returns outputs that carry an autograd node (`_FusedTrainFn`);
@@ -7,6 +7,7 @@ Two ways in, both replacing trainer.py:153-161 (`outputs = model(inputs)`, `mt_l
     kernel launch that writes every parameter gradient.  Two launches per step.
   * `train_step(model, inputs, labels, tasks, lambdas, log_sigmas)`: forward + multi-task loss + backward in a
     SINGLE cooperative kernel launch; `.grad` of every parameter (and of log_sigmas) is populated directly.
+    LocoModel only: MultiTaskLoss indexes LocoModel's output columns, and MonolocoModel trains through the drop-in.
 Optimizer / clip_grad_norm_ / scheduler stay PyTorch (trainer.py:159-161).
 """
 import ctypes as C
@@ -20,17 +21,32 @@ from .. import _lib as L_
 _WS = weakref.WeakKeyDictionary()
 
 
+def _is_loco(model):
+    from ..network.architectures import LocoModel
+    return isinstance(model, LocoModel)
+
+
 def _blocks_of(model):
-    """(name of Linear, name of BatchNorm or None, res_src) in forward order (architectures.py:48-71)."""
+    """(name of Linear, name of BatchNorm or None, res_src) in forward order: LocoModel (architectures.py:48-71) ends
+    with the BatchNorm-free w2 and w3; MonolocoModel (:135-176) ends with its last stage, whose residual the head reads."""
     blocks = [('w1', 'batch_norm1', -1)]
     src = 0
     for i in range(model.num_stage):
         blocks.append(('linear_stages.%d.w1' % i, 'linear_stages.%d.batch_norm1' % i, -1))
         blocks.append(('linear_stages.%d.w2' % i, 'linear_stages.%d.batch_norm2' % i, src))
         src = len(blocks) - 1
-    blocks.append(('w2', None, -1))
-    blocks.append(('w3', 'batch_norm3', -1))
+    if _is_loco(model):
+        blocks.append(('w2', None, -1))
+        blocks.append(('w3', 'batch_norm3', -1))
     return blocks
+
+
+def _heads_of(model):
+    """(input size, aux head or None, final head, output columns): LocoModel's out = [w_fin | w_aux]; MonolocoModel's
+    out = w2 (no aux head, mlb_train_args.aux_block = -1)."""
+    if _is_loco(model):
+        return model.stereo_size, 'w_aux', 'w_fin', model.output_size + 1
+    return model.input_size, None, 'w2', model.output_size
 
 
 class _Workspace:
@@ -39,10 +55,11 @@ class _Workspace:
         self.h = C.c_void_p()
         self.max_rows = max_rows
         self.blocks = _blocks_of(model)
+        self.in_size, self.aux, self.fin, self.out_cols = _heads_of(model)
         self.lambda_cache = {}
         self.generation = 0   # bumped by every launch that overwrites the saved activations (forward / train_step)
         L_.check(self.lib.mlb_train_create(device.index if device.index is not None else torch.cuda.current_device(),
-                                           max_rows, model.stereo_size, model.linear_size, len(self.blocks),
+                                           max_rows, self.in_size, model.linear_size, len(self.blocks),
                                            C.byref(self.h)), 'mlb_train_create')
 
     def __del__(self):
@@ -87,8 +104,8 @@ def _fill(model, ws, x, out, grads=None, g_out=None, labels=None, tasks=None, sc
             if grads is not None:
                 b.dgamma, b.dbeta = grads[bn + '.weight'].data_ptr(), grads[bn + '.bias'].data_ptr()
     a = L_.MlbTrainArgs()
-    a.n_rows, a.input_size, a.output_size = x.shape[0], model.stereo_size, model.output_size + 1
-    a.linear_size, a.n_blocks, a.aux_block = model.linear_size, nb, nb - 2
+    a.n_rows, a.input_size, a.output_size = x.shape[0], ws.in_size, ws.out_cols
+    a.linear_size, a.n_blocks, a.aux_block = model.linear_size, nb, nb - 2 if ws.aux else -1
     a.update_running_stats = int(update_running)
     a.rows_per_group = int(os.environ.get('MLB_TRAIN_ROWS_PER_GROUP', '0'))  # 0 = auto; tests sweep 8..16
     a.p_dropout, a.bn_eps, a.bn_momentum = float(model.p_dropout), 1e-5, 0.1
@@ -96,11 +113,15 @@ def _fill(model, ws, x, out, grads=None, g_out=None, labels=None, tasks=None, sc
     if drop_mask is not None:
         a.drop_mask = drop_mask.data_ptr()
     a.x, a.out = x.data_ptr(), out.data_ptr()
-    a.W_aux, a.b_aux = model.w_aux.weight.data_ptr(), model.w_aux.bias.data_ptr()
-    a.W_fin, a.b_fin = model.w_fin.weight.data_ptr(), model.w_fin.bias.data_ptr()
+    fin = _mod(model, ws.fin)
+    a.W_fin, a.b_fin = fin.weight.data_ptr(), fin.bias.data_ptr()
     if grads is not None:
-        a.dW_aux, a.db_aux = grads['w_aux.weight'].data_ptr(), grads['w_aux.bias'].data_ptr()
-        a.dW_fin, a.db_fin = grads['w_fin.weight'].data_ptr(), grads['w_fin.bias'].data_ptr()
+        a.dW_fin, a.db_fin = grads[ws.fin + '.weight'].data_ptr(), grads[ws.fin + '.bias'].data_ptr()
+    if ws.aux:   # MonolocoModel: no aux head, its pointers stay NULL
+        aux = _mod(model, ws.aux)
+        a.W_aux, a.b_aux = aux.weight.data_ptr(), aux.bias.data_ptr()
+        if grads is not None:
+            a.dW_aux, a.db_aux = grads[ws.aux + '.weight'].data_ptr(), grads[ws.aux + '.bias'].data_ptr()
     if g_out is not None:
         a.g_out = g_out.data_ptr()
     if labels is not None:
@@ -121,9 +142,15 @@ def _stream(device):
 
 
 def _check_model(model, x):
-    from ..network.architectures import LocoModel
-    if not isinstance(model, LocoModel):
-        raise NotImplementedError("fused training supports the LocoModel topology (what Trainer builds, trainer.py:115)")
+    from ..network.architectures import LocoModel, MonolocoModel
+    if not isinstance(model, (LocoModel, MonolocoModel)):
+        raise NotImplementedError("fused training supports the LocoModel and MonolocoModel topologies")
+    if isinstance(model, MonolocoModel):
+        # 1 + 2 num_stage blocks; the kernel takes 2..MLB_MAX_BLOCKS (16) of them and at most 16 output columns
+        if not 1 <= model.num_stage <= 7:
+            raise ValueError("fused training of MonolocoModel needs num_stage in [1, 7] (got %d)" % model.num_stage)
+        if not 1 <= model.output_size <= 16:
+            raise ValueError("fused training of MonolocoModel needs output_size in [1, 16] (got %d)" % model.output_size)
     if not x.is_cuda or next(model.parameters()).device != x.device:
         raise RuntimeError("monoloco_b200 training runs on CUDA tensors only (no CPU fallback)")
     if x.shape[0] < 2:
@@ -142,7 +169,7 @@ class _FusedTrainFn(torch.autograd.Function):
     def forward(ctx, x, model, seed, drop_mask, *params):
         ws = _workspace(model, x.shape[0], x.device)
         x = x.detach().float().contiguous()
-        out = torch.empty((x.shape[0], model.output_size + 1), dtype=torch.float32, device=x.device)
+        out = torch.empty((x.shape[0], ws.out_cols), dtype=torch.float32, device=x.device)
         a, blocks = _fill(model, ws, x, out, drop_seed=seed, drop_mask=drop_mask)
         L_.check(ws.lib.mlb_train_forward(ws.h, C.byref(a), blocks, _stream(x.device)), 'mlb_train_forward')
         _bump_batches_tracked(model)
@@ -197,8 +224,13 @@ def fused_train_forward(model, x, drop_mask=None, seed=None):
 def train_step(model, x, labels, tasks, lambdas=None, log_sigmas=None, drop_mask=None, seed=None, accumulate=False):
     """Forward + MultiTaskLoss (losses.py:59-73; AutoTune :28-43 when log_sigmas is given) + backward in ONE kernel
     launch.  Populates `.grad` of every model parameter (and of log_sigmas); returns (loss, [weighted task losses])
-    exactly like `mt_loss(model(x), labels, phase='train')` followed by `loss.backward()`."""
+    exactly like `mt_loss(model(x), labels, phase='train')` followed by `loss.backward()`.  LocoModel only."""
     _check_model(model, x)
+    if not _is_loco(model):
+        raise NotImplementedError(
+            "train_step() fuses MultiTaskLoss, which reads LocoModel's output columns (process.py:231-254); the reference "
+            "defines no multi-task loss for MonolocoModel's outputs.  Train MonolocoModel through the drop-in instead: "
+            "out = model(x) in train mode, any loss built in torch from `out`, loss.backward() (two launches).")
     if seed is None:
         seed = _next_drop_seed(x.device)
     tasks = tuple(tasks)
@@ -206,7 +238,7 @@ def train_step(model, x, labels, tasks, lambdas=None, log_sigmas=None, drop_mask
     ws = _workspace(model, x.shape[0], x.device)
     x = x.detach().float().contiguous()
     labels = labels.detach().float().contiguous()
-    out = torch.empty((x.shape[0], model.output_size + 1), dtype=torch.float32, device=x.device)
+    out = torch.empty((x.shape[0], ws.out_cols), dtype=torch.float32, device=x.device)
     # task weights as a device tensor (cached per lambdas; AutoTune's depend on log_sigmas and are computed on the device):
     # no host<->device synchronisation anywhere in the step, so consecutive steps queue back to back
     lam = ws.lambda_cache.get(lambdas)
