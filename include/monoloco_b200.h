@@ -367,6 +367,49 @@ int mlb_adam_clip_step(int n_tensors, float* const* params, const float* const* 
                        float beta1, float beta2, float eps, float weight_decay, int64_t step, double* sqnorm_scratch_dev,
                        void* stream);
 
+/* ---- loss statistics of the train / validate / evaluate loop (trainer.py:165-167,193-197,250-284) -------------
+ * From (outputs, labels) of n_seg CSR row segments, ADDS into acc[seg][MLB_STATS_NACC] (fp64, device), so one buffer
+ * can hold a whole epoch of batches. One CTA per segment, a fixed row-to-thread map and a fixed reduction tree, no float
+ * atomics: the same inputs give the same bits. Columns as extract_outputs / extract_labels (process.py:231-297):
+ * out = [x, y, d, log b, h, w, l, sin, cos(, aux)], labels = [x, y, z, d, h, w, l, sin, cos, yaw(, aux)].
+ * Per segment (sums over its rows unless stated):
+ *   MLB_STAT_N          rows
+ *   MLB_STAT_TOTAL      rows * MultiTaskLoss / AutoTuneMultiTaskLoss train-form loss (losses.py:28-73): the weighted
+ *                       sum of the task means (Laplace NLL for d, L1 for x y h w l ori, BCE-with-logits for aux) plus,
+ *                       with log_sigmas, sum(log_sigmas); weights lambda_t or lambda_t / (2 exp(log_sigma_t)^2) with
+ *                       log_sigmas read from device memory when the kernel runs
+ *   MLB_STAT_VAL + t    the val-form losses (losses.py:76-101) of task t (MLB_TASK_*): |d - d_gt| (l1_loss_from_laplace),
+ *                       |o - o_gt| for x y h w l, |atan2(sin, cos) - atan2(sin_gt, cos_gt)| in radians for ori (the
+ *                       caller applies * 180 / 3.14), BCE-with-logits for aux
+ *   MLB_STAT_BI         bi = exp(log b) * d (unnormalize_bi)
+ *   MLB_STAT_BI_HIT     rows with |d - d_gt| <= bi (both in fp32, as the reference compares them)
+ *   MLB_STAT_ERR/_ERR2  |d - d_gt| and its square (unbiased std on the host)
+ *   MLB_STAT_AUX_MISS   |(sigmoid(aux) >= 0.5) - aux_gt| (fp32 sigmoid), only with MLB_TASK_AUX in task_mask
+ *   MLB_STAT_LAPLACE    Laplace NLL |1 - d / d_gt| exp(-log b) + 0.01 + log b + 2
+ *   MLB_STAT_ORI_L1     |sin - sin_gt| + |cos - cos_gt| (the train-form ori L1 divides it by 2 rows)
+ * A segment of 0 rows adds nothing. */
+#define MLB_STATS_MAX_SEG 16
+#define MLB_STATS_NACC 17
+enum { MLB_STAT_N = 0, MLB_STAT_TOTAL = 1, MLB_STAT_VAL = 2, MLB_STAT_BI = 10, MLB_STAT_BI_HIT = 11, MLB_STAT_ERR = 12,
+       MLB_STAT_ERR2 = 13, MLB_STAT_AUX_MISS = 14, MLB_STAT_LAPLACE = 15, MLB_STAT_ORI_L1 = 16 };
+
+typedef struct mlb_task_stats_args {
+    int32_t n_seg;                         /* 1..MLB_STATS_MAX_SEG                                               */
+    int32_t out_cols;                      /* 9 (mono) or 10 (stereo)                                            */
+    int32_t label_ld;                      /* 10 (mono) or 11 (stereo); MLB_TASK_AUX needs 10 / 11               */
+    int32_t task_mask;                     /* bit t set for MLB_TASK_t; bits 0..7 only                           */
+    int32_t seg_off[MLB_STATS_MAX_SEG + 1]; /* host values: rows of segment s are seg_off[s] .. seg_off[s+1]-1, */
+                                           /* seg_off[0] >= 0 and non-decreasing                                */
+    int32_t reserved;                      /* must be 0                                                          */
+    float lambdas[8];                      /* train-form task weight by task id                                  */
+    const float* out;                      /* [seg_off[n_seg]][out_cols] device                                  */
+    const float* labels;                   /* [seg_off[n_seg]][label_ld] device                                  */
+    const float* log_sigmas;               /* AutoTune: [popcount(task_mask)] device, in task-id order; or NULL  */
+    double* acc;                           /* [n_seg][MLB_STATS_NACC] device, added to                          */
+} mlb_task_stats_args;
+/* Asynchronous on `stream`, one launch; rejects bad arguments with mlb_last_error() before launching. */
+int mlb_task_stats(const mlb_task_stats_args* args, void* stream);
+
 /* ---- NVLink peer buffers for the fused all-gather (cudaIpc*, one process per GPU) ---- */
 #define MLB_IPC_HANDLE_BYTES 64
 /* cudaMalloc `bytes` on `device` (zero-filled) and export an IPC handle for the other ranks. */

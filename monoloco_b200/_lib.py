@@ -26,7 +26,7 @@ KERNEL_NAMES = {0: 'loco_forward_kernel (FFMA row tiles)', 1: 'loco_forward_clus
 EXPORTS = ['mlb_create', 'mlb_update_weights', 'mlb_destroy', 'mlb_last_error', 'mlb_abi_version', 'mlb_num_sms', 'mlb_device_error', 'mlb_last_kernel', 'mlb_tc_resident_clusters', 'mlb_kernel_times',
            'mlb_forward', 'mlb_forward_host', 'mlb_forward_images', 'mlb_preprocess', 'mlb_stereo_filter', 'mlb_stereo_filter_images', 'mlb_post_process', 'mlb_kitti_rows', 'mlb_social_distance', 'mlb_raising_hand', 'mlb_decode', 'mlb_laplace_std', 'mlb_ipc_alloc', 'mlb_ipc_open', 'mlb_ipc_close', 'mlb_ipc_free', 'mlb_train_create', 'mlb_train_destroy',
            'mlb_train_forward', 'mlb_train_backward', 'mlb_train_step', 'mlb_train_phase_times', 'mlb_train_subphase_times',
-           'mlb_adam_clip_step',
+           'mlb_adam_clip_step', 'mlb_task_stats',
            'mlb_probe_ffma',
            'mlb_launch_count', 'mlb_debug_fwd_marks',
            ]
@@ -103,6 +103,18 @@ class MlbTrainArgs(C.Structure):
                 ('task_scale_dev', C.c_void_p)]
 
 
+STATS_MAX_SEG = 16
+STATS_NACC = 17
+STAT_N, STAT_TOTAL, STAT_VAL, STAT_BI, STAT_BI_HIT, STAT_ERR, STAT_ERR2, STAT_AUX_MISS, STAT_LAPLACE, STAT_ORI_L1 = \
+    0, 1, 2, 10, 11, 12, 13, 14, 15, 16
+
+
+class MlbTaskStatsArgs(C.Structure):
+    _fields_ = [('n_seg', C.c_int32), ('out_cols', C.c_int32), ('label_ld', C.c_int32), ('task_mask', C.c_int32),
+                ('seg_off', C.c_int32 * (STATS_MAX_SEG + 1)), ('reserved', C.c_int32), ('lambdas', C.c_float * 8),
+                ('out', C.c_void_p), ('labels', C.c_void_p), ('log_sigmas', C.c_void_p), ('acc', C.c_void_p)]
+
+
 _lib = None
 
 
@@ -156,6 +168,7 @@ def lib():
     l.mlb_adam_clip_step.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int64,
                                      C.c_void_p, C.c_void_p]
+    l.mlb_task_stats.argtypes = [C.POINTER(MlbTaskStatsArgs), C.c_void_p]
     l.mlb_probe_ffma.argtypes = [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double), C.c_void_p]
     l.mlb_launch_count.restype = C.c_uint64
     if l.mlb_abi_version() != MLB_ABI_VERSION:

@@ -191,3 +191,36 @@ def make_crowd(n, seed=0, spacing=(0.3, 3.0)):
     dds = [math.hypot(x, z) * float(rng.uniform(0.95, 1.05)) for x, z in centers]
     stds = rng.uniform(0.2, 1.0, n).tolist()
     return centers, angles, dds, stds
+
+
+TRAINER_CLUSTERS = (('10', 0, 10), ('20', 10, 20), ('30', 20, 30), ('40', 30, 40), ('>40', 40, 1e9))
+
+
+def make_trainer_joints(path, n_train=600, n_val=150, stereo=False, seed=11):
+    """A joints file for Trainer runs: inputs like normalised keypoints, labels with the reference's column meaning
+    (x, y, z, d, h, w, l, sin, cos, yaw(, aux)), d in [2, 48) m so that every cluster 10 / 20 / 30 / 40 has rows."""
+    import json
+    rng = np.random.RandomState(seed)
+    dic = {'version': 'synthetic-trainer-1'}
+    for phase, n in (('train', n_train), ('val', n_val)):
+        X = rng.uniform(-1.5, 1.5, size=(n, 68 if stereo else 34))
+        d = rng.uniform(2, 48, size=n)
+        yaw = rng.uniform(-math.pi, math.pi, size=n)
+        # a learnable signal: the first input columns carry the targets up to noise
+        X[:, 0] = d / 16 - 1.5 + rng.normal(0, 0.05, n)
+        X[:, 1] = np.sin(yaw) + rng.normal(0, 0.05, n)
+        cols = [rng.uniform(-0.6, 0.6, n), rng.uniform(-0.2, 0.2, n), d * 0.95, d, rng.uniform(1.4, 2.0, n),
+                rng.uniform(0.4, 0.9, n), rng.uniform(0.4, 1.2, n), np.sin(yaw), np.cos(yaw), yaw]
+        if stereo:
+            cols.append(rng.randint(0, 2, n).astype(np.float64))
+        Y = np.stack(cols, 1)
+        clst = {}
+        for name, lo, hi in TRAINER_CLUSTERS:
+            sel = [i for i in range(n) if lo <= Y[i, 3] < hi]
+            clst[name] = {'X': X[sel].tolist(), 'Y': Y[sel].tolist()}
+        kps = rng.uniform(0, 1000, size=(n, 3, 17))
+        dic[phase] = {'X': X.tolist(), 'Y': Y.tolist(), 'names': ['%06d.png' % i for i in range(n)],
+                      'kps': kps.tolist(), 'clst': clst}
+    with open(path, 'w') as f:
+        json.dump(dic, f)
+    return dic

@@ -2,3 +2,5 @@ from .losses import LaplacianLoss, MultiTaskLoss, AutoTuneMultiTaskLoss, Composi
 from .fused import train_step, fused_train_forward
 from .optim import FusedClipAdam
 from .datasets import KeypointsDataset, DeviceLoader
+from .stats import task_stats
+from .trainer import Trainer
