@@ -19,11 +19,14 @@
 //                and only 30 four-CTA clusters fit an H100 at once (120 of 132 SMs; a 4096 batch then takes three rounds
 //                of tiles instead of two).
 //   per tile     prologue: thread = row: pre-process the raw keypoints (process.py:47-67 / 25-44) straight into hi / lo planes
-//                per layer: the producer warp streams the stages through a 4-slot ring (lane 0) and stages the layer's
-//                epilogue constants (the other lanes); consumer warpgroup c issues 2 k-steps x 3 wgmma (M 64, N 128, K 8)
-//                per stage on output columns [128c, 128c + 128) and releases the stage once its wgmma group retired.
+//                per layer: the producer lane streams the stages through a 4-slot ring, running ahead of the consumers
+//                within a tile (a layer's W planes while the previous layer finishes, its X planes once the group barrier
+//                publishes them) and bulk-copies the layer's epilogue constants into one of two buffers; consumer
+//                warpgroup c issues 2 k-steps x 3 wgmma (M 64, N 128, K 8) per stage on output columns [128c, 128c + 128)
+//                and releases the stage once its wgmma group retired.
 //                Two 64 x 128 accumulators per warpgroup = 128 registers per thread: a 128-row tile would need twice that.
-//                The summed accumulators go through shared memory (the idle ring) to a thread = (row, 64 columns) epilogue:
+//                The summed accumulators go through shared memory (the layer's last two ring slots, held until read) to a
+//                thread = (row, 64 columns) epilogue:
 //                folded BN / ReLU / dropout / residual, written straight into the next layer's hi / lo planes; narrow heads
 //                (w_aux, w_fin, MonolocoModel.w2) are accumulated on the CUDA cores from the same registers;
 //                a group barrier (tc_group_sync: counter in global memory) separates the layers
@@ -51,12 +54,13 @@ constexpr int TC_MAX_CT = 8;       // column tiles = CTAs per group (L <= 2048)
 constexpr int TC_HW = 16;          // head output columns in total (output_size <= 16)
 constexpr int TC_EPI = 256;        // consumer threads: 2 warpgroups (wgmma), then the epilogue, thread = (row, 64 columns)
 constexpr int TC_THREADS = TC_EPI + 32;   // + the producer warp (TMA ring, epilogue constants)
-constexpr int TC_SLD = TCN + 8;    // row stride (floats) of the accumulator staging tile: conflict-free float2 stores
+constexpr int TC_SLD = TCWN + 8;   // row stride (floats) of a warpgroup's staging tile: conflict-free float2 stores
 constexpr size_t TC_RING_BYTES = (size_t)TCNST * TC_STAGE;                      // 160 KB
 constexpr size_t TC_SST_BYTES = 2 * TCN * sizeof(float);                        // folded-BN scale | shift of the layer
 constexpr size_t TC_HW_BYTES = (size_t)TC_HW * TCN * sizeof(float);             // head weights of the layer
-constexpr size_t TC_SMEM_BYTES = TC_RING_BYTES + TC_SST_BYTES + TC_HW_BYTES;    // 178 KB
-static_assert((size_t)TCM * TC_SLD * sizeof(float) <= TC_RING_BYTES, "accumulator staging aliases the ring");
+constexpr size_t TC_CONST_BYTES = TC_SST_BYTES + TC_HW_BYTES;                   // one buffer of epilogue constants
+constexpr size_t TC_SMEM_BYTES = TC_RING_BYTES + 2 * TC_CONST_BYTES;            // 196 KB: two constant buffers
+static_assert((size_t)TCM * TC_SLD * sizeof(float) <= TC_STAGE, "a warpgroup's staging tile fits one ring slot");
 static_assert((size_t)4 * TC_MAX_CT * TCM * TC_HW * sizeof(float) <= TC_RING_BYTES, "head partials alias the ring");
 
 struct TcExtra {
@@ -104,7 +108,10 @@ __device__ __forceinline__ void tc_fence_regs(float* d) {
     for (int i = 0; i < TCWN / 2; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 __device__ __forceinline__ void tc_consumer_sync() { asm volatile("bar.sync 2, 256;" ::: "memory"); }   // the 2 consumer warpgroups
-__device__ __forceinline__ void tc_layer_sync() { asm volatile("bar.sync 1, 288;" ::: "memory"); }      // + the producer warp
+__device__ __forceinline__ void tc_warpgroup_sync(int wg) {   // one consumer warpgroup (named barriers 3 and 4)
+    if (wg == 0) asm volatile("bar.sync 3, 128;" ::: "memory");
+    else asm volatile("bar.sync 4, 128;" ::: "memory");
+}
 
 constexpr int TC_ERR_GROUP_TIMEOUT = 3;                       // the error word's "grid barrier" code
 constexpr unsigned long long TC_GROUP_TIMEOUT_NS = 20000000000ull;
@@ -151,6 +158,38 @@ __device__ __forceinline__ void tc_group_sync(TcGroupBar* gb, int* err_flag) {
     if (threadIdx.x == 0) tc_group_wait(gb, err_flag);
     __syncthreads();
 }
+// The per-layer barrier: the CTA-level halves are over the 256 consumer threads only (the producer warp runs ahead into the
+// next layer).  Thread 0 then hands the published X planes to the producer lane through the shared mbarrier `xpub` (one
+// phase per layer barrier); the producer runs fence.proxy.async before its TMA reads them.  A dead group still arrives, so
+// the producer is released.
+__device__ __forceinline__ void tc_group_sync_consumers(TcGroupBar* gb, int* err_flag, uint64_t* xpub) {
+    tc_consumer_sync();
+    if (threadIdx.x == 0) {
+        tc_group_wait(gb, err_flag);
+        mbar_arrive(xpub);
+    }
+    tc_consumer_sync();
+}
+// Producer-warp wait on a hand-off that can lie behind a group barrier: backs off like mbar_wait_backoff, but is bounded by
+// %globaltimer at twice the group-barrier timeout, so that a stalled peer ends the kernel through the barrier's error code
+// (the barrier's own timeout always arrives first) rather than through this wait.
+__device__ __forceinline__ void tc_wait_behind_group(uint64_t* bar, uint32_t parity, int* err_flag) {
+    unsigned long long t0 = 0;
+    for (unsigned spins = 1; !mbar_try_wait(bar, parity); ++spins) {
+        __nanosleep(128);
+        if ((spins & 255u) == 0) {
+            unsigned long long t;
+            asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+            if (t0 == 0) {
+                t0 = t;
+            } else if (t - t0 > 2 * TC_GROUP_TIMEOUT_NS) {
+                if (err_flag) *reinterpret_cast<volatile int*>(err_flag) = ERR_MBAR_TIMEOUT;
+                __threadfence_system();
+                __trap();
+            }
+        }
+    }
+}
 // thread 0, before its first arrival: base = the counter before this launch.  Every earlier launch left it at a multiple of
 // nct, and the peers of this launch can be at most nct - 1 arrivals past it (barrier 0 needs this CTA's arrival).
 __device__ __forceinline__ void tc_group_init(TcGroupBar* gb, unsigned long long* ctr) {
@@ -182,7 +221,8 @@ __global__ void tc_pack_weights_kernel(const float* __restrict__ wt, float* __re
 
 // profiling aid (mlb_debug_fwd_marks): CTA (0,0) stamps %globaltimer per layer of its first tile: thread 0 at [8g+0] layer start,
 // [8g+3] accumulators complete, [8g+4] epilogue done, [8g+5] group barrier passed; MMA lane at [8g+1] first stage landed,
-// [8g+2] all MMAs issued; producer lane at [8g+6] all stages issued.  Per tile t < 4 of group 0, thread 0: [128+4t] tile
+// [8g+2] all MMAs issued; producer lane at [8g+6] all stages issued, [8g+7] X copies of the layer issued (the X planes of
+// layers g >= 1 wait for the group barrier of layer g-1; their W planes do not).  Per tile t < 4 of group 0, thread 0: [128+4t] tile
 // start, [129+4t] prologue barrier passed, [130+4t] head partials gathered, [131+4t] rows stored.  Group barriers per tile:
 // one after the prologue, one per layer (the last one also publishes the head partials).
 __device__ unsigned long long* g_tc_marks = nullptr;
@@ -193,6 +233,12 @@ __device__ __forceinline__ void tmark(unsigned long long* marks, int slot) {
         marks[slot] = t;
     }
 }
+
+struct TcHeadGroups {     // the narrow heads' rows grouped by the GEMM layer that feeds them (g = 0, 1)
+    int src[2];           // op index of the feeding layer (-1: no group)
+    int q0[2], n[2];      // first head row, row count
+    int nq[2], off[2];    // rows rounded up to 4, first hacc slot
+};
 
 struct TcEpi {            // what one epilogue pass over this thread's 64 columns needs
     const float* acc;     // shared: this thread's row of the staged accumulators (main + cross), at its first column
@@ -323,16 +369,20 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                                                                         const __grid_constant__ TcExtra ex,
                                                                         const __grid_constant__ ImgParams ib) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    __shared__ __align__(8) uint64_t full[TCNST], empty[TCNST];
+    // full[s]: two arrivals per fill (the W planes as soon as the slot is empty, the X planes once they are published);
+    // empty[s]: one arrival per consumer warp.  cready / cfree[b]: epilogue-constant buffer b staged / read.  xpub: the
+    // X planes of the next layer are published (thread 0, after the group barrier) -> the producer lane.
+    __shared__ __align__(8) uint64_t full[TCNST], empty[TCNST], cready[2], cfree[2], xpub;
     __shared__ TcGroupBar gbar;
+    __shared__ TcHeadGroups hgrp;   // kept in shared memory, out of the registers of the MMA loop
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int nt = blockIdx.y, nct = gridDim.y, L = p.L;
     const bool epi_thread = tid < TC_EPI, prod_warp = tid >= TC_EPI, prod_lane = tid == TC_EPI;
     const int wg = (tid >> 7) & 1;     // consumer warpgroup: output columns [128 wg, 128 wg + 128) of the CTA's 256
-    const int quarter = (tid >> 6) & 3;   // epilogue threads: which 64 columns of the CTA's 256
-    float* sst = reinterpret_cast<float*>(smem_raw + TC_RING_BYTES);                 // [2][256]
-    float* hw = reinterpret_cast<float*>(smem_raw + TC_RING_BYTES + TC_SST_BYTES);   // [TC_HW][256]
-    float* stg = reinterpret_cast<float*>(smem_raw);     // [64][TC_SLD] summed accumulators of the layer; aliases the idle ring
+    const int quarter = (tid >> 6) & 3;   // epilogue threads: which 64 columns of the CTA's 256 (quarters 2 wg, 2 wg + 1)
+    // two buffers of epilogue constants, each scale | shift [2][256] then head weights [TC_HW][256]: layer g's buffer is
+    // refilled at layer g+2, so the producer lane's copies never wait on the epilogue that reads the other one
+    float* cbuf = reinterpret_cast<float*>(smem_raw + TC_RING_BYTES);
     float* hpart = reinterpret_cast<float*>(smem_raw);   // [4 nct][64][TC_HW] on CTA 0; aliases the idle ring
 
     // this group's workspace slot
@@ -347,31 +397,42 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
 
     if (tid == 0) {
         // every consumer warp releases a stage once its warpgroup's wgmma reading it have retired
-        for (int s = 0; s < TCNST; ++s) mbar_init(&full[s], 1), mbar_init(&empty[s], TC_EPI / 32);
+        for (int s = 0; s < TCNST; ++s) mbar_init(&full[s], 2), mbar_init(&empty[s], TC_EPI / 32);
+        // cready: the producer lane's bulk copies (expect_tx) + the 31 other producer lanes' zero rows
+        for (int b = 0; b < 2; ++b) mbar_init(&cready[b], 32), mbar_init(&cfree[b], TC_EPI / 32);
+        mbar_init(&xpub, 1);
         mbar_fence_init();
         // after the residual: [4 nct][64][TC_HW] head partials of every CTA of the group, then the barrier counter
         tc_group_init(&gbar, reinterpret_cast<unsigned long long*>(res + (size_t)TCM * L + (size_t)4 * nct * TCM * TC_HW));
+        // head rows are grouped by the layer that feeds them (at most two groups: w_aux | w_fin, or MonolocoModel.w2);
+        // group g accumulates into hacc[off_g .. off_g + nq_g), nq_g = its row count rounded up to 4 (zero weights
+        // beyond the real rows)
+        int src[2] = {-1, -1}, q0[2] = {0, 0}, n[2] = {0, 0};
+        for (int q = 0; q < ex.n_head_rows; ++q) {
+            const int g = (src[0] < 0 || src[0] == ex.head_src[q]) ? 0 : 1;
+            if (n[g] == 0) src[g] = ex.head_src[q], q0[g] = q;
+            n[g]++;
+        }
+        for (int g = 0; g < 2; ++g) hgrp.src[g] = src[g], hgrp.q0[g] = q0[g], hgrp.n[g] = n[g], hgrp.nq[g] = (n[g] + 3) & ~3;
+        hgrp.off[0] = 0, hgrp.off[1] = hgrp.nq[0];
     }
     __syncthreads();
+    const int* grp_src = hgrp.src;
+    const int* grp_q0 = hgrp.q0;
+    const int* grp_n = hgrp.n;
+    const int* grp_nq = hgrp.nq;
+    const int* grp_off = hgrp.off;
 
     const float zm = p.z_met;
     const float k0 = p.kinv[0], k1 = p.kinv[1], k2 = p.kinv[2], k3 = p.kinv[3], k4 = p.kinv[4], k5 = p.kinv[5];
     const bool mc_drop = (p.flags & MLB_FWD_DROPOUT) != 0;
-    // head rows are grouped by the layer that feeds them (at most two groups: w_aux | w_fin, or MonolocoModel.w2); group g
-    // accumulates into hacc[off_g .. off_g + nq_g), nq_g = its row count rounded up to 4 (zero weights beyond the real rows)
-    int grp_src[2] = {-1, -1}, grp_q0[2] = {0, 0}, grp_n[2] = {0, 0};
-    for (int q = 0; q < ex.n_head_rows; ++q) {
-        const int g = (grp_src[0] < 0 || grp_src[0] == ex.head_src[q]) ? 0 : 1;
-        if (grp_n[g] == 0) grp_src[g] = ex.head_src[q], grp_q0[g] = q;
-        grp_n[g]++;
-    }
     int n_gemm = 0;
     for (int oi = 0; oi < p.n_ops; ++oi) n_gemm += p.ops[oi].type == MLB_OP_GEMM;
-    const int grp_nq[2] = {(grp_n[0] + 3) & ~3, (grp_n[1] + 3) & ~3};
-    const int grp_off[2] = {0, grp_nq[0]};
 
     unsigned long long* marks = (blockIdx.x == 0 && blockIdx.y == 0 && (tid == 0 || prod_lane)) ? g_tc_marks : nullptr;
-    unsigned it_p = 0, it_m = 0;  // stages issued / consumed so far (producer lane, consumer warpgroups)
+    // ring stages and GEMM layers of the layers before this thread's current one (the producer warp is ahead of the
+    // consumers, each counts its own): stage it uses slot it % TCNST, layer n uses constant buffer n & 1
+    unsigned it0 = 0, n_lay = 0;
     float acc_m[TCWN / 2], acc_c[TCWN / 2];   // this thread's wgmma fragments: main (a_hi.w_hi) and cross terms
     for (int rb = (int)blockIdx.x; rb < ex.n_tiles; rb += (int)gridDim.x) {
         unsigned long long* tmk = (tid == 0 && rb < 4 * (int)gridDim.x) ? marks : nullptr;   // group 0's first four tiles
@@ -460,44 +521,78 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
             const mlb_op& op = p.ops[oi];
             if (op.type != MLB_OP_GEMM) continue;
             const int n_kb = ex.n_kb[oi];
-            const float* xsrc_f = gi == 0 ? xin : xpl[par];
+            // this layer's X planes and head group (-1: none), evaluated where used: neither stays live across the MMAs
+            auto x_src = [&]() { return reinterpret_cast<const unsigned char*>(gi == 0 ? xin : xpl[par]); };
+            auto head_group = [&]() { return grp_src[0] == oi ? 0 : (grp_src[1] == oi ? 1 : -1); };
             unsigned long long* mk = (rb == 0 && gi < 15) ? marks : nullptr;
             if (tid == 0) tmark(mk, 8 * gi + 0);
-            const int hg = grp_src[0] == oi ? 0 : (grp_src[1] == oi ? 1 : -1);   // head group fed by this layer
-            const bool head_layer = hg >= 0;
+            auto const_buf = [&](unsigned n) { return cbuf + (size_t)(n & 1) * (TC_CONST_BYTES / sizeof(float)); };
 
             if (prod_lane) {
-                // ---- producer: this row tile's X planes and this column tile's W planes, 40 KB per stage
-                asm volatile("fence.proxy.async;" ::: "memory");  // peers' generic-proxy stores (planes, hpart) -> async-proxy TMA
-                const unsigned char* xsrc = reinterpret_cast<const unsigned char*>(xsrc_f);
+                // ---- producer: this row tile's X planes and this column tile's W planes, 40 KB per stage.  Within a tile
+                // this lane runs ahead of the consumers: the W planes of a layer's first stages do not depend on the
+                // activations, so they stream while the previous layer's last MMAs, epilogue and group barrier run (its
+                // staging tile sits in the other two slots); the X planes follow once thread 0 hands them over (xpub).
+                const unsigned char* xsrc = x_src();
                 const unsigned char* wsrc = reinterpret_cast<const unsigned char*>(ex.wplanes[oi]) + (size_t)nt * n_kb * 2 * TC_W_PLANE;
-                for (int kb = 0; kb < n_kb; ++kb, ++it_p) {
-                    const unsigned s = it_p % TCNST;
-                    if (it_p >= TCNST) mbar_wait(&empty[s], ((it_p / TCNST) - 1) & 1, p.err_flag);
-                    unsigned char* st = smem_raw + (size_t)s * TC_STAGE;
-                    mbar_expect_tx(&full[s], TC_STAGE);
-                    tma_bulk_g2s(st, xsrc + (size_t)kb * 2 * TC_A_PLANE, 2 * TC_A_PLANE, &full[s]);
-                    tma_bulk_g2s(st + 2 * TC_A_PLANE, wsrc + (size_t)kb * 2 * TC_W_PLANE, 2 * TC_W_PLANE, &full[s]);
+                auto fill_w = [&](int kb) {
+                    const unsigned it = it0 + kb, s = it % TCNST;
+                    if (it >= TCNST) mbar_wait(&empty[s], ((it / TCNST) - 1) & 1, p.err_flag);
+                    mbar_expect_tx(&full[s], 2 * TC_W_PLANE);
+                    tma_bulk_g2s(smem_raw + (size_t)s * TC_STAGE + 2 * TC_A_PLANE, wsrc + (size_t)kb * 2 * TC_W_PLANE, 2 * TC_W_PLANE, &full[s]);
+                };
+                auto fill_x = [&](int kb) {   // after fill_w(kb): the slot is empty
+                    const unsigned s = (it0 + kb) % TCNST;
+                    mbar_expect_tx(&full[s], 2 * TC_A_PLANE);
+                    tma_bulk_g2s(smem_raw + (size_t)s * TC_STAGE, xsrc + (size_t)kb * 2 * TC_A_PLANE, 2 * TC_A_PLANE, &full[s]);
+                };
+                int kb = 0;
+                if (gi > 0)
+                    for (; kb < n_kb && kb < TCNST; ++kb) fill_w(kb);
+                // xpub: one phase per layer barrier (layer 0 of a tile follows the CTA-wide prologue barrier, which is
+                // later than the previous tile's last phase)
+                if (n_lay > 0) tc_wait_behind_group(&xpub, (n_lay - 1) & 1, p.err_flag);
+                // the prologue barrier (layer 0) or xpub ordered the peers' generic-proxy stores (planes, hpart) before
+                // this point: -> async-proxy TMA
+                asm volatile("fence.proxy.async;" ::: "memory");
+                for (int k = 0; k < kb; ++k) fill_x(k);
+                if (kb == 0) fill_w(0), fill_x(0), kb = 1;
+                tmark(mk, 8 * gi + 7);
+                {
+                    // this layer's epilogue constants, as bulk copies into buffer n_lay & 1 (every blob array is 128-byte
+                    // aligned): folded-BN scale | shift and the real rows of the head group fed here.  Issued here, the
+                    // copies neither delay the layer's first X copies nor stall this lane behind global loads.
+                    const unsigned b = n_lay & 1;
+                    float* sst = const_buf(n_lay);
+                    const int hg = head_group();
+                    const int nrow = hg >= 0 ? grp_n[hg] : 0;
+                    if (n_lay >= 2) mbar_wait(&cfree[b], ((n_lay >> 1) - 1) & 1, p.err_flag);
+                    mbar_expect_tx(&cready[b], (uint32_t)(2 + nrow) * TCN * sizeof(float));
+                    tma_bulk_g2s(sst, p.blob + op.scale_off + nt * TCN, TCN * sizeof(float), &cready[b]);
+                    tma_bulk_g2s(sst + TCN, p.blob + op.shift_off + nt * TCN, TCN * sizeof(float), &cready[b]);
+                    for (int r = 0; r < nrow; ++r)
+                        tma_bulk_g2s(sst + (2 + r) * TCN, p.blob + ex.head_w[grp_q0[hg] + r] + nt * TCN, TCN * sizeof(float), &cready[b]);
                 }
+                for (; kb < n_kb; ++kb) fill_w(kb), fill_x(kb);
                 tmark(mk, 8 * gi + 6);
             } else if (prod_warp) {
-                // ---- the other producer lanes, while the MMAs run: this layer's epilogue constants -> shared memory
-                const int st = lane - 1;   // 0 .. 30
-                for (int i = st; i < 2 * TCN; i += 31)
-                    sst[i] = __ldg(p.blob + (i < TCN ? op.scale_off : op.shift_off) + nt * TCN + (i & (TCN - 1)));
-                if (head_layer) {
-                    for (int i = st; i < grp_nq[hg] * TCN; i += 31) {
-                        const int r = i / TCN, c = i % TCN;
-                        hw[i] = r < grp_n[hg] ? __ldg(p.blob + ex.head_w[grp_q0[hg] + r] + nt * TCN + c) : 0.f;
-                    }
-                }
+                // ---- the other producer lanes: zero head-weight rows beyond the real ones (rows rounded up to 4) in this
+                // layer's constant buffer, once the epilogue two layers back has read it.  Stores only: global loads on
+                // these lanes stalled the producer lane that shares their warp (its first copies by up to 28 us, or
+                // the MMA stream, in tools/tc_marks.py), so the constants themselves come by bulk copy.
+                float* hw = const_buf(n_lay) + 2 * TCN;   // [TC_HW][256]
+                const int hg = head_group();
+                if (n_lay >= 2) tc_wait_behind_group(&cfree[n_lay & 1], ((n_lay >> 1) - 1) & 1, p.err_flag);
+                if (hg >= 0)
+                    for (int i = grp_n[hg] * TCN + lane - 1; i < grp_nq[hg] * TCN; i += 31) hw[i] = 0.f;
+                mbar_arrive(&cready[n_lay & 1]);
             } else {
                 // ---- consumer warpgroup wg: 2 k-steps x 3 wgmma (M 64, N 128, K 8) per stage, one stage in flight
 #pragma unroll
                 for (int i = 0; i < TCWN / 2; ++i) acc_m[i] = 0.f, acc_c[i] = 0.f;
-                for (int kb = 0; kb < n_kb; ++kb, ++it_m) {
-                    const unsigned s = it_m % TCNST;
-                    mbar_wait(&full[s], (it_m / TCNST) & 1, p.err_flag);
+                for (int kb = 0; kb < n_kb; ++kb) {
+                    const unsigned it = it0 + kb, s = it % TCNST;
+                    mbar_wait(&full[s], (it / TCNST) & 1, p.err_flag);
                     if (kb == 0 && tid == 0) tmark(mk, 8 * gi + 1);
                     const uint32_t a_hi = smem_u32(smem_raw + (size_t)s * TC_STAGE), a_lo = a_hi + TC_A_PLANE;
                     const uint32_t w_hi = a_hi + 2 * TC_A_PLANE + (uint32_t)wg * (TCWN / 8) * TC_SBO, w_lo = w_hi + TC_W_PLANE;
@@ -513,17 +608,21 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                     tc_wgmma_commit();
                     tc_wgmma_wait<1>();   // the previous stage's group has retired: release its slot
                     tc_fence_regs(acc_m), tc_fence_regs(acc_c);
-                    if (kb > 0 && lane == 0) mbar_arrive(&empty[(it_m - 1) % TCNST]);
+                    // the layer's last two stages stay held: their slots take the staging tiles (released after the epilogue)
+                    if (kb > 0 && kb + 1 < n_kb && lane == 0) mbar_arrive(&empty[(it - 1) % TCNST]);
                 }
                 tc_wgmma_wait<0>();
                 tc_fence_regs(acc_m), tc_fence_regs(acc_c);
-                if (lane == 0) mbar_arrive(&empty[(it_m - 1) % TCNST]);
                 if (tid == 0) tmark(mk, 8 * gi + 2);
                 tc_consumer_sync();   // both warpgroups are done reading the ring: stage the accumulators over it
+                // warpgroup wg stages its 64 x 128 summed accumulators into the slot of this layer's stage n - 2 + wg
+                // (n = it0 + n_kb, n_kb >= 2), which is the next layer's stage n + 2 + wg: the producer fills that layer's
+                // first two stages meanwhile.  The warpgroup's epilogue threads (quarters 2 wg, 2 wg + 1) read only this tile.
+                float* stg = reinterpret_cast<float*>(smem_raw + (size_t)((it0 + n_kb + 2 + wg) % TCNST) * TC_STAGE);   // [64][TC_SLD]
                 {
                     // fragment of wgmma m64nNk8: warp w of the warpgroup holds rows 16w .. 16w + 15; lane l rows
                     // 16w + l/4 (+ 8), columns 8g + 2 (l % 4) (+ 1) of every 8-column group g
-                    const int r0 = 16 * (warp & 3) + (lane >> 2), c0 = TCWN * wg + 2 * (lane & 3);
+                    const int r0 = 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
                     for (int g = 0; g < TCWN / 8; ++g) {
                         float* d = stg + (size_t)r0 * TC_SLD + c0 + 8 * g;
@@ -533,11 +632,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                     }
                 }
             }
-            __syncwarp();
-            tc_layer_sync();   // staged accumulators and epilogue constants are complete
             if (epi_thread) {
+                const float* stg = reinterpret_cast<const float*>(smem_raw + (size_t)((it0 + n_kb + 2 + wg) % TCNST) * TC_STAGE);
+                tc_warpgroup_sync(wg);                                         // my warpgroup's staging tile is complete
+                mbar_wait(&cready[n_lay & 1], (n_lay >> 1) & 1, p.err_flag);   // this layer's epilogue constants are staged
+                const int hg = head_group();
+                const bool head_layer = hg >= 0;
                 TcEpi e;
-                e.sst = sst, e.hw = hw, e.nxt = xpl[gi == 0 ? 0 : (par ^ 1)], e.res = res;
+                e.sst = const_buf(n_lay), e.hw = e.sst + 2 * TCN, e.nxt = xpl[gi == 0 ? 0 : (par ^ 1)], e.res = res;
                 e.tid = row, e.grow = grow, e.site = site, e.live = live;
                 e.relu = (op.flags & MLB_F_RELU) != 0, e.add_res = (op.flags & MLB_F_ADD_RES) != 0;
                 e.save_res = (op.flags & MLB_F_SAVE_RES) != 0, e.drop = mc_drop && (op.flags & MLB_F_DROPOUT) != 0;
@@ -548,7 +650,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                 e.keep = tc_policy_evict_last();
                 if (tid == 0) tmark(mk, 8 * gi + 3);
                 e.ccol0 = TCH * quarter, e.col0 = nt * TCN + TCH * quarter;
-                e.acc = stg + (size_t)row * TC_SLD + e.ccol0;
+                e.acc = stg + (size_t)row * TC_SLD + TCH * (quarter & 1);
                 float hacc[TC_HW];   // head partial sums over my 64 columns; slots [off, off + nq) of the group fed here
 #pragma unroll
                 for (int q = 0; q < TC_HW; ++q) hacc[q] = 0.f;
@@ -586,28 +688,41 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                     for (int q4 = 0; q4 < TC_HW / 4; ++q4)
                         if (q4 >= q4a && q4 < q4b) dst[q4] = make_float4(hacc[4 * q4], hacc[4 * q4 + 1], hacc[4 * q4 + 2], hacc[4 * q4 + 3]);
                 }
+                // the staging tile and the constants are read: the two held slots go back to the producer lane (this
+                // thread's generic-proxy accesses ordered before its async-proxy refills) and the constant buffer to the
+                // other producer lanes
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                __syncwarp();
+                if (lane == 0) {
+                    mbar_arrive(&empty[(it0 + n_kb - 2) % TCNST]);
+                    mbar_arrive(&empty[(it0 + n_kb - 1) % TCNST]);
+                    mbar_arrive(&cfree[n_lay & 1]);
+                }
                 if (tid == 0) tmark(mk, 8 * gi + 4);
-            }
-            if (op.flags & MLB_F_DROPOUT) site++;
-            tc_group_sync(&gbar, p.err_flag);   // all column tiles of this row tile are written; the staging tile has been read
-            if (tid == 0) tmark(mk, 8 * gi + 5);
-            // The planes this layer read are dead now (every CTA of the group is past its MMAs) and will be fully
-            // rewritten before their next use: drop the dirty lines from L2 instead of letting them be written back to
-            // HBM (discard.global.L2; without it the workspace churn was 255 MB of DRAM writes per batch of 4096).
-            {
+                // all column tiles of this row tile are written; then the X planes of the next layer go to the producer
+                tc_group_sync_consumers(&gbar, p.err_flag, &xpub);
+                if (tid == 0) tmark(mk, 8 * gi + 5);
+                // The planes this layer read are dead now (every CTA of the group is past its MMAs) and will be fully
+                // rewritten before their next use: drop the dirty lines from L2 instead of letting them be written back to
+                // HBM (discard.global.L2; without it the workspace churn was 255 MB of DRAM writes per batch of 4096).
                 const size_t lines = (size_t)n_kb * 2 * TC_A_PLANE / 128;   // 128-byte lines; CTA nt takes lines nt, nt + nct, ...
-                const unsigned char* base = reinterpret_cast<const unsigned char*>(xsrc_f);
-                for (size_t ln = (size_t)nt + (size_t)nct * tid; ln < lines; ln += (size_t)nct * TC_THREADS)
+                const unsigned char* base = x_src();
+                for (size_t ln = (size_t)nt + (size_t)nct * tid; ln < lines; ln += (size_t)nct * TC_EPI)
                     asm volatile("discard.global.L2 [%0], 128;" ::"l"(base + ln * 128) : "memory");
                 if ((op.flags & MLB_F_ADD_RES) && !(op.flags & MLB_F_SAVE_RES)) {   // last use of the stage residual
                     const unsigned char* rb = reinterpret_cast<const unsigned char*>(res + (size_t)(nt * TCN / 4) * TCM * 4);
-                    for (size_t o = (size_t)tid * 128; o < (size_t)TCN * TCM * 4; o += (size_t)TC_THREADS * 128)
+                    for (size_t o = (size_t)tid * 128; o < (size_t)TCN * TCM * 4; o += (size_t)TC_EPI * 128)
                         asm volatile("discard.global.L2 [%0], 128;" ::"l"(rb + o) : "memory");
                 }
             }
+            if (op.flags & MLB_F_DROPOUT) site++;
             if (gi > 0) par ^= 1;
-            ++gi;
+            ++gi, ++n_lay, it0 += n_kb;
         }
+        // the producer warp rejoins: the tail aliases the ring (hpart) and the constants (gather staging), and the last
+        // layer's group barrier ordered the peers' head partials before this point
+        __syncwarp();
+        __syncthreads();
 
         // ------------------------------------------------------------ tail: head partials (slot) -> CTA 0 -> decode + stores
         // the head layers wrote every CTA's partials to the slot; the last layer's group barrier ordered them before this point
@@ -630,16 +745,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) loco_forward_tc_kernel(const __
                 for (int t = 0; t < 4 * nct; ++t) s += hpart[((size_t)t * TCM + row) * TC_HW + slot];  // fixed order: deterministic
                 o[ex.head_col[q]] = s + __ldg(p.blob + ex.head_b[q]);
             }
-            store_row<IMAGES>(p, (size_t)grow, o, cenrow, p.n_gather ? hw + (size_t)row * MLB_GATHER_LD : nullptr, &ib);
+            store_row<IMAGES>(p, (size_t)grow, o, cenrow, p.n_gather ? cbuf + (size_t)row * MLB_GATHER_LD : nullptr, &ib);
         }
         if (nt == 0 && p.n_gather) {
             // fused all-gather: the tile's rows ([<=64][20] floats, contiguous in every gather buffer) leave as coalesced
             // 16-byte stores -- 128-byte NVLink packets instead of 11 scattered 4..16-byte stores per row and peer
-            // (`hw` is free here: the head layers are done; it is re-staged in the next tile's first head layer)
+            // (the constant buffers are free here: the tile's layers are done; the next tile stages them after its
+            // prologue barrier)
             __syncthreads();
             const int rows_live = min(TCM, p.n_rows - rb * TCM);
             const int n4 = rows_live * (MLB_GATHER_LD / 4);
-            const float4* src = reinterpret_cast<const float4*>(hw);
+            const float4* src = reinterpret_cast<const float4*>(cbuf);
             for (int pg = 0; pg < p.n_gather; ++pg) {
                 float4* dst = reinterpret_cast<float4*>(p.gather[pg] + (size_t)(p.gather_row0 + (long long)rb * TCM) * MLB_GATHER_LD);
                 for (int i = tid; i < n4; i += TC_THREADS) dst[i] = src[i];
@@ -690,6 +806,8 @@ mlb_tc_state* mlb_tc_prepare(const float* blob_dev, const mlb_op* ops, int n_ops
         if (ops[i].type != MLB_OP_GEMM) continue;
         if (first < 0) first = i;
         t->n_kb[i] = (ops[i].Kpad + TCKB - 1) / TCKB;
+        // at least two k blocks (zero-padded): a layer's last two ring slots take the accumulator staging tiles
+        if (t->n_kb[i] < 2) t->n_kb[i] = 2;
         const size_t fl = (size_t)2 * t->n_kb[i] * TCKB * L;
         if ((*err = cudaMalloc(&t->wplanes[i], fl * sizeof(float))) != cudaSuccess) return nullptr;
         tc_pack_weights_kernel<<<264, 256, 0, st>>>(blob_dev + ops[i].w_off, t->wplanes[i], ops[i].Kpad, L, t->n_kb[i]);

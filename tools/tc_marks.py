@@ -29,12 +29,14 @@ print('B=%d: %d tiles of 64 rows on %d co-resident CTA groups of 4 CTAs = %d til
 t0 = m[128]
 print('first tile of group 0, per layer (us from the layer start; layer start from the tile start):')
 for g in range(15):
-    s, first, issued, acc, epi, bar, prod = m[8 * g:8 * g + 7]
+    s, first, issued, acc, epi, bar, prod, xiss = m[8 * g:8 * g + 8]
     if s == 0:
         break
-    print('  layer %d @%7.1f: first stage +%5.1f | MMAs issued +%5.1f | accumulators done +%5.1f | epilogue end +%5.1f | '
-          'group barrier +%5.1f | producer done +%5.1f' % (g, (s - t0) / 1e3, (first - s) / 1e3, (issued - s) / 1e3, (acc - s) / 1e3,
-                                                           (epi - s) / 1e3, (bar - s) / 1e3, (prod - s) / 1e3))
+    # the producer lane runs ahead: its marks of layer g can precede the layer's start on thread 0 (negative)
+    print('  layer %d @%7.1f: X copies issued %+6.1f | first stage +%5.1f | MMAs issued +%5.1f | accumulators done +%5.1f | '
+          'epilogue end +%5.1f | group barrier +%5.1f | producer done %+6.1f' % (
+              g, (s - t0) / 1e3, (xiss - s) / 1e3, (first - s) / 1e3, (issued - s) / 1e3, (acc - s) / 1e3, (epi - s) / 1e3,
+              (bar - s) / 1e3, (prod - s) / 1e3))
 print('tiles of group 0 (us from the kernel\'s first mark):')
 for t in range(4):
     start, pro, heads, stored = m[128 + 4 * t:132 + 4 * t]
