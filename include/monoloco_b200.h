@@ -272,6 +272,36 @@ int mlb_social_distance(const mlb_social_args* args, void* stream);
 /* is_raising_hand for n poses kps [n][3][17] fp64 (device): out[i] = 0 none, 1 left, 2 right, 3 both. */
 int mlb_raising_hand(const double* kps, int n, int8_t* out, void* stream);
 
+/* ---- preprocess_pifpaf for a BATCH of images (process.py:155-207): pifpaf annotations -> boxes [x1, y1, x2, y2, conf]
+ * and key points [3][17], bit for bit with the reference's Python floats (fp64 in its operation order; the keypoint-
+ * confidence mean in numpy's pairwise order for 17 values).  Annotations of all images are concatenated (ann_off CSR).
+ * The kept ones (conf >= min_conf) are compacted image-major, each image in its original order.  One launch, one CTA per
+ * image; no host synchronisation.  The reference's `assert delta_h > -5 and delta_w > -5` (annotations without a score)
+ * sets bit 0 of *error; bit 1 marks a time-out of the kept-offset scan (2 s).  Outputs have room for n_ann rows; read
+ * kept_off[n_img] for the kept count.  All pointers are device pointers. */
+typedef struct mlb_pifpaf_args {
+    int32_t n_img;             /* >= 1                                                                               */
+    int32_t n_ann;             /* annotations over all images                                                        */
+    int32_t enlarge;           /* 1 (enlarge_boxes=True) or 2 (False)                                                */
+    int32_t reserved;
+    double min_conf;           /* finite                                                                             */
+    const int32_t* ann_off;    /* [n_img + 1] annotations of image i are [ann_off[i], ann_off[i+1])                 */
+    const double* kps;         /* [n_ann][51] dic['keypoints'] (x, y, c per joint)                                   */
+    const double* bbox;        /* [n_ann][4] dic['bbox']                                                             */
+    const double* score;       /* [n_ann] dic['score'] where has_score[k], or NULL with has_score NULL              */
+    const uint8_t* has_score;  /* [n_ann] 1 if the annotation has a 'score' key; NULL: none has                       */
+    const double* im_size;     /* [n_img][2] width, height where has_size[i], or NULL with has_size NULL            */
+    const uint8_t* has_size;   /* [n_img] 1 if image i has a size (boxes clamped into it); NULL: none has           */
+    double* out_boxes;         /* [n_ann][5] kept boxes x1, y1, x2, y2, conf                                         */
+    double* out_kps;           /* [n_ann][3][17] kept key points (xs, ys, confs)                                     */
+    float* out_kps32;          /* [n_ann][3][17] the same in fp32 (the network's input)                              */
+    int32_t* out_src;          /* [n_ann] index of each kept row's annotation                                        */
+    int32_t* kept_off;         /* [n_img + 1] kept rows of image i are [kept_off[i], kept_off[i+1])                 */
+    int32_t* error;            /* [1] error word, zeroed by the call                                                 */
+    uint64_t* scratch;         /* [n_img + 1] scan state, zeroed by the call                                         */
+} mlb_pifpaf_args;
+int mlb_preprocess_pifpaf(const mlb_pifpaf_args* args, void* stream);
+
 /* decode only (process.py:231-278 / 330-360 on a raw tensor that did not come from mlb_forward):
  * raw [B, out_size] -> dec [B, 8] as in mlb_forward_args.out_dec.  Device buffers. */
 int mlb_decode(const float* raw, int n_rows, int out_size, int decode_kind, float* dec, void* stream);

@@ -24,7 +24,7 @@ KERNEL_NAMES = {0: 'loco_forward_kernel (FFMA row tiles)', 1: 'loco_forward_clus
                 4: 'loco_forward_wide2_kernel (FFMA, 4-CTA clusters, K x N split)'}
 
 EXPORTS = ['mlb_create', 'mlb_update_weights', 'mlb_destroy', 'mlb_last_error', 'mlb_abi_version', 'mlb_num_sms', 'mlb_device_error', 'mlb_last_kernel', 'mlb_tc_resident_clusters', 'mlb_kernel_times',
-           'mlb_forward', 'mlb_forward_host', 'mlb_forward_images', 'mlb_preprocess', 'mlb_stereo_filter', 'mlb_stereo_filter_images', 'mlb_post_process', 'mlb_kitti_rows', 'mlb_social_distance', 'mlb_raising_hand', 'mlb_decode', 'mlb_laplace_std', 'mlb_ipc_alloc', 'mlb_ipc_open', 'mlb_ipc_close', 'mlb_ipc_free', 'mlb_train_create', 'mlb_train_destroy',
+           'mlb_forward', 'mlb_forward_host', 'mlb_forward_images', 'mlb_preprocess', 'mlb_stereo_filter', 'mlb_stereo_filter_images', 'mlb_post_process', 'mlb_kitti_rows', 'mlb_social_distance', 'mlb_raising_hand', 'mlb_preprocess_pifpaf', 'mlb_decode', 'mlb_laplace_std', 'mlb_ipc_alloc', 'mlb_ipc_open', 'mlb_ipc_close', 'mlb_ipc_free', 'mlb_train_create', 'mlb_train_destroy',
            'mlb_train_forward', 'mlb_train_backward', 'mlb_train_step', 'mlb_train_phase_times', 'mlb_train_subphase_times',
            'mlb_adam_clip_step', 'mlb_task_stats',
            'mlb_probe_ffma',
@@ -76,6 +76,17 @@ class MlbSocialArgs(C.Structure):
                 ('threshold_prob', C.c_double), ('threshold_dist', C.c_double), ('radii', C.c_double * SOCIAL_MAX_RADII),
                 ('img_off', C.c_void_p), ('xz', C.c_void_p), ('angles', C.c_void_p), ('dds', C.c_void_p),
                 ('stds', C.c_void_p), ('table', C.c_void_p), ('out', C.c_void_p)]
+
+
+class MlbPifpafArgs(C.Structure):
+    _fields_ = [('n_img', C.c_int32), ('n_ann', C.c_int32), ('enlarge', C.c_int32), ('reserved', C.c_int32),
+                ('min_conf', C.c_double), ('ann_off', C.c_void_p), ('kps', C.c_void_p), ('bbox', C.c_void_p),
+                ('score', C.c_void_p), ('has_score', C.c_void_p), ('im_size', C.c_void_p), ('has_size', C.c_void_p),
+                ('out_boxes', C.c_void_p), ('out_kps', C.c_void_p), ('out_kps32', C.c_void_p), ('out_src', C.c_void_p),
+                ('kept_off', C.c_void_p), ('error', C.c_void_p), ('scratch', C.c_void_p)]
+
+
+PIFPAF_ERR_BOX, PIFPAF_ERR_TIMEOUT = 1, 2   # bits of mlb_pifpaf_args.error
 
 
 MLB_MAX_BLOCKS = 16
@@ -152,6 +163,7 @@ def lib():
                                  C.c_void_p]
     l.mlb_social_distance.argtypes = [C.POINTER(MlbSocialArgs), C.c_void_p]
     l.mlb_raising_hand.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    l.mlb_preprocess_pifpaf.argtypes = [C.POINTER(MlbPifpafArgs), C.c_void_p]
     l.mlb_decode.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     l.mlb_laplace_std.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p]
     l.mlb_ipc_alloc.argtypes = [C.c_int, C.c_size_t, C.POINTER(C.c_void_p), C.c_char_p]

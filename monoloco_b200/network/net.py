@@ -204,6 +204,168 @@ class Loco:
             res[i] = dic
         return res
 
+    def predict_batch(self, annotations_list, kk_list, im_size_list, *, annotations_r_list=None, dic_gt_list=None,
+                      enlarge_boxes=False, min_conf=0., iou_min=0.3, reorder=True, activities=(), args=None):
+        """The reference's per-image predict chain (predict.py:226-240, eval/eval_activity.py:173-179) for many images:
+        res[i] = (boxes, keypoints, dic_out) of
+            boxes, keypoints = preprocess_pifpaf(annotations_list[i], im_size_list[i], enlarge_boxes, min_conf)
+            dic_out = post_process(forward(keypoints, kk_list[i][, keypoints_r]), boxes, keypoints, kk_list[i], dic_gt_list[i],
+                                   iou_min, reorder)
+            then social_distance(dic_out, args) if 'social_distance' in activities, raising_hand(dic_out, keypoints) if
+            'raise_hand' in activities,
+        with keypoints_r from preprocess_pifpaf(annotations_r_list[i], im_size_list[i]) in stereo (predict.py:244).
+        Every stage is a device launch over all images: the pre-process (mlb_preprocess_pifpaf, left and right), the
+        network (forward_images, the stereo filter, MC-dropout when n_dropout > 0), mlb_post_process, social distancing
+        on the people in post-processed order and raised hands on the kept key points in caller order.  The annotations
+        go up in one copy; the host waits twice: for the kept counts (they size the network launch) and for the results.
+        The annotation dictionaries are not modified.  Raises AssertionError for the reference's degenerate-box assert
+        (nothing after the pre-process is launched) and ValueError for bad arguments or where the reference's Laplace
+        constructor would fail in social_distance."""
+        import numpy as np
+        from ..engine import image_offsets, kinv_images
+        from .process import check_pifpaf_options, pack_pifpaf, pifpaf_layout, preprocess_pifpaf_device
+        from .post import (post_process_device, gt_arrays, assemble_post, social_distance_device, raising_hand_device,
+                           check_laplace_args, RAISING_HAND)
+        n_img = len(annotations_list)
+        if len(kk_list) != n_img or len(im_size_list) != n_img:
+            raise ValueError("predict_batch: one camera matrix and one image size (or None) per image")
+        if dic_gt_list is not None and len(dic_gt_list) != n_img:
+            raise ValueError("predict_batch: one ground truth (or None) per image")
+        stereo = self.net == 'monstereo'
+        if annotations_r_list is not None and (not stereo or len(annotations_r_list) != n_img):
+            raise ValueError("predict_batch: annotations_r_list is for stereo, one list per image")
+        enlarge, min_conf = check_pifpaf_options(enlarge_boxes, min_conf)
+        acts = tuple(activities)
+        if set(acts) - {'social_distance', 'raise_hand'}:
+            raise ValueError("predict_batch: activities are 'social_distance' and 'raise_hand'")
+        want_sd, want_rh = 'social_distance' in acts, 'raise_hand' in acts
+        if want_sd and (args is None or self.net == 'monoloco'):
+            raise ValueError("predict_batch: social_distance needs args and a net with orientation outputs")
+        packs = [pack_pifpaf(annotations_list, im_size_list)]
+        if stereo:
+            packs.append(pack_pifpaf(annotations_r_list if annotations_r_list is not None else [[]] * n_img, im_size_list))
+        gt = gt_arrays(dic_gt_list) if dic_gt_list is not None else None
+
+        def finish(res, flags=None, codes=None):   # social_distance / raising_hand in the reference's order
+            if want_sd:
+                res['angles'], res['dds_pred'], res['stds_ale'], res['xyz_pred']  # noqa: B018  (the reads create the keys)
+                res['social_distance'] = flags if flags is not None else []
+            if want_rh:
+                res['raising_hand'] = codes if codes is not None else []
+            return res
+
+        if n_img == 0:
+            return []
+        if sum(int(p['ann_off'][-1]) for p in packs) == 0:
+            return [([], [], finish(defaultdict(list))) for _ in range(n_img)]
+        dev, eng = self.device, self.model.engine()
+        with torch.no_grad():
+            # ---- one upload of everything the pre-process reads, the pre-process, one read-back of the kept counts
+            lays, nbytes = pifpaf_layout(packs)
+            h_in = _pinned_host('pb_in', (nbytes,), torch.uint8)
+            hn = h_in.numpy()
+            for p, lay in zip(packs, lays):
+                for name, (o, shape, dt) in lay.items():
+                    a = np.ascontiguousarray(p[name], dtype=dt).reshape(-1).view(np.uint8)
+                    hn[o:o + a.size] = a
+            d_in = h_in.to(dev, non_blocking=True)
+            tdt = {np.dtype(np.float64): torch.float64, np.dtype(np.int32): torch.int32, np.dtype(np.uint8): torch.uint8}
+            pre = []
+            for k, (p, lay) in enumerate(zip(packs, lays)):
+                arrays = {name: d_in[o:o + int(np.prod(shape)) * dt.itemsize].view(tdt[dt]).view(shape)
+                          for name, (o, shape, dt) in lay.items()}
+                pre.append(preprocess_pifpaf_device(arrays, n_img, p['kps'].shape[0], *((enlarge, min_conf) if k == 0 else
+                                                                                      (1, 0.))))
+            h_rb = _pinned_host('pb_rb', (len(pre), n_img + 2), torch.int32)
+            for k, o in enumerate(pre):
+                h_rb[k, :n_img + 1].copy_(o['kept_off'], non_blocking=True)
+                h_rb[k, n_img + 1:].copy_(o['error'], non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+            rb = h_rb.numpy().astype(np.int64)
+            if (rb[:, -1] & L_.PIFPAF_ERR_TIMEOUT).any():
+                raise RuntimeError("mlb_preprocess_pifpaf: the kept-offset scan timed out")
+            if (rb[:, -1] & L_.PIFPAF_ERR_BOX).any():
+                raise AssertionError("Bounding box <=0")
+            koff = rb[0, :n_img + 1]
+            n_l = np.diff(koff)
+            n = int(koff[-1])
+            if n == 0:
+                return [([], [], finish(defaultdict(list))) for _ in range(n_img)]
+
+            # ---- network
+            kps32 = pre[0]['kps32'][:n]
+            epi = None
+            if stereo:
+                n_r = np.diff(rb[1, :n_img + 1])
+                n_re = np.where(n_l > 0, np.maximum(n_r, 1), 0)   # no right poses: the first left pose (net.py:115-116)
+                n_rt = int(rb[1, n_img])
+                src = np.concatenate([np.arange(rb[1, i], rb[1, i + 1]) if n_r[i] else [n_rt + koff[i]]
+                                      for i in range(n_img) if n_l[i]]).astype(np.int64)
+                x_right = torch.cat((pre[1]['kps32'][:n_rt], kps32)).index_select(0, torch.from_numpy(src).to(dev))
+                row_off, right_off = image_offsets(n_l * n_re), image_offsets(n_re)
+                out = eng.forward_images(kps32, row_off, kk_list, kind=L_.IN_KPS_STEREO, x_right=x_right, left_off=koff,
+                                         right_off=right_off, want_xyzc=True)
+                sel = eng.stereo_filter_images(out['raw'], out['dec'], row_off, koff, right_off, xyzc=out['xyzc'], trim=False)
+                # post_process reads the first n_l rows of every image's filtered outputs (net.py:195-201)
+                img = np.repeat(np.arange(n_img), n_l)
+                local = np.arange(n) - koff[img]
+                rows = torch.from_numpy(np.stack((img, local))).to(dev)
+                gidx = (sel['sel_img_off'].long()[rows[0]] + rows[1]).clamp_(max=max(out['raw'].shape[0] - 1, 0))
+                dec = sel['sel_dec'].index_select(0, gidx)
+            else:
+                zc = self.net == 'monoloco'
+                dec = eng.forward_images(kps32, koff, kk_list, kind=L_.IN_KPS, want_xyzc=True, zero_center=zc)['dec']
+                if self.n_dropout > 0:
+                    epi = eng.epistemic_std(kps32, self.n_dropout, n_samples=self.N_SAMPLES, seed=1, row_off=koff,
+                                            kk_list=kk_list, zero_center=zc)
+
+            # ---- post-process, activities
+            up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev, non_blocking=True)  # noqa: E731
+            gt_dev = {k: up(v) if isinstance(v, np.ndarray) else v for k, v in gt.items()} if gt else None
+            dev_out = post_process_device(pre[0]['kept_off'], pre[0]['boxes'][:n], kps32, up(kinv_images(kk_list)), dec,
+                                          int(n_l.max()), gt=gt_dev, iou_min=iou_min, reorder=reorder)
+            dev_out.update(dec=dec, boxes=pre[0]['boxes'][:n], kps=pre[0]['kps'][:n])
+            if epi is not None:
+                dev_out['epi'] = epi
+            if want_sd:   # social_interactions(idx, ...) over dic_out['xyz_pred'], i.e. in post-processed order
+                gidx = up(np.repeat(koff[:-1], n_l)) + dev_out['order'].long()
+                xyz_o, dec_o = dev_out['xyz'].index_select(0, gidx), dec.index_select(0, gidx)
+                dev_out['sd'] = social_distance_device(xyz_o[:, [0, 2]], dec_o[:, 5], dec_o[:, 3], dec_o[:, 4], koff,
+                                                       threshold_prob=args.threshold_prob,
+                                                       threshold_dist=args.threshold_dist, radii=args.radii,
+                                                       n_samples=self.N_SAMPLES)
+            if want_rh:   # net.py:267-271: the key points as preprocess_pifpaf returned them
+                dev_out['rh'] = raising_hand_device(dev_out['kps'])
+
+            # ---- one download of every result
+            h = {}
+            for k, v in dev_out.items():
+                h[k] = _pinned_host('pb_' + k, tuple(v.shape), v.dtype)
+                h[k].copy_(v, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+        eng.check_error()
+        h = {k: v.numpy() for k, v in h.items()}
+        dd, bi = h['dec'][:, 3].astype(np.float64), h['dec'][:, 4].astype(np.float64)
+        if want_sd:
+            check_laplace_args(dd, bi)   # laplace_sampling (process.py:101-122) in social_interactions
+        epi = h['epi'].astype(np.float64) if 'epi' in h else np.zeros(n)
+        has_yaw, has_aux = self.net != 'monoloco', stereo
+        boxes, kps = h['boxes'].tolist(), h['kps'].tolist()
+        sd = h['sd'].tolist() if want_sd else None
+        rh = [RAISING_HAND[c] for c in h['rh'].tolist()] if want_rh else None
+        results = []
+        for i in range(n_img):
+            a, b = int(koff[i]), int(koff[i + 1])
+            res = defaultdict(list)
+            if b > a:
+                yaw = (h['dec'][a:b, 5].astype(np.float64), h['dec'][a:b, 6].astype(np.float64)) if has_yaw else None
+                assemble_post(res, {k: h[k][a:b] for k in ('xyz', 'conf', 'uv', 'match', 'order', 'xyz_real')},
+                              int(h['n_match'][i]), boxes[a:b], kps[a:b], dd[a:b], bi[a:b], epi[a:b], yaw,
+                              h['dec'][a:b, 7].astype(np.float64) if has_aux else None,
+                              dic_gt_list[i] if dic_gt_list is not None else None)
+            results.append((boxes[a:b], kps[a:b], finish(res, sd[a:b] if want_sd else None, rh[a:b] if want_rh else None)))
+        return results
+
     def _pinned(self, name, shape, dtype):
         """Pinned host buffer of this Loco, reused across calls (each call synchronises before it returns)."""
         import math

@@ -27,17 +27,15 @@ def post_process_batch(items, iou_min=0.3, reorder=True, device=None):
     None; a `dic_in` of None yields an empty dictionary).  Returns the list of per-image result dictionaries."""
     if not torch.cuda.is_available():
         raise RuntimeError("monoloco_b200: no CUDA device -- post_process_batch has no CPU fallback")
-    lib = L_.lib()
     dev = torch.device('cuda', torch.cuda.current_device()) if device is None else torch.device(device)
     live = [i for i, it in enumerate(items) if it[0] is not None and len(it[1]) > 0]
     results = [defaultdict(list) for _ in items]
     if not live:
         return results
-    det_off, gt_off = [0], [0]
-    boxes, kps, kinv, dec, gtb, gtd = [], [], [], [], [], []
-    any_gt = False
+    det_off = [0]
+    boxes, kps, kinv, dec = [], [], [], []
     for i in live:
-        dic_in, bx, kp, kk, dic_gt = items[i]
+        dic_in, bx, kp, kk, _ = items[i]
         m = len(bx)
         det_off.append(det_off[-1] + m)
         boxes.append(np.asarray(bx, dtype=np.float64).reshape(m, 5))
@@ -47,78 +45,101 @@ def post_process_batch(items, iou_min=0.3, reorder=True, device=None):
         d[:, 3] = np.asarray(dic_in['d'], dtype=np.float32).reshape(-1)
         d[:, 4] = np.asarray(dic_in['bi'], dtype=np.float32).reshape(-1)
         dec.append(d)
-        if dic_gt and len(dic_gt['boxes']):
-            any_gt = True
-            g = len(dic_gt['boxes'])
-            gtb.append(np.asarray(dic_gt['boxes'], dtype=np.float64).reshape(g, -1)[:, :4])
-            gtd.append(np.asarray([y[3] for y in dic_gt['ys']], dtype=np.float64))
-            gt_off.append(gt_off[-1] + g)
-        else:
-            gt_off.append(gt_off[-1])
-    M = det_off[-1]
+    gt = gt_arrays([items[i][4] for i in live])
     t = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a)).to(dev, dtype=dt)  # noqa: E731
-    d_boxes = t(np.concatenate(boxes), torch.float64)
-    d_kps = t(np.concatenate(kps), torch.float32)
-    d_kinv = t(np.stack(kinv), torch.float32)
-    d_dec = t(np.concatenate(dec), torch.float32)
-    d_doff = t(np.asarray(det_off, dtype=np.int32), torch.int32)
-    d_goff = t(np.asarray(gt_off, dtype=np.int32), torch.int32) if any_gt else None
-    d_gtb = t(np.concatenate(gtb), torch.float64) if any_gt else None
-    d_gtd = t(np.concatenate(gtd), torch.float64) if any_gt else None
-    o_xyz = torch.empty((M, 3), dtype=torch.float32, device=dev)
-    o_ray = torch.empty((M, 4), dtype=torch.float32, device=dev)
-    o_conf = torch.empty((M,), dtype=torch.float64, device=dev)
-    o_uv = torch.empty((M, 6), dtype=torch.int32, device=dev)
-    o_match = torch.empty((M,), dtype=torch.int32, device=dev)
-    o_order = torch.empty((M,), dtype=torch.int32, device=dev)
-    o_nm = torch.empty((len(live),), dtype=torch.int32, device=dev)
-    o_xr = torch.zeros((M, 3), dtype=torch.float32, device=dev)
-    p = lambda x: x.data_ptr() if x is not None else None  # noqa: E731
-    a = L_.MlbPostArgs(len(live), max(det_off[i + 1] - det_off[i] for i in range(len(live))),
-                       max(gt_off[i + 1] - gt_off[i] for i in range(len(live))), int(bool(reorder)), float(iou_min),
-                       p(d_doff), p(d_goff), p(d_boxes), p(d_kps), p(d_kinv), p(d_dec), p(d_gtb), p(d_gtd), p(o_xyz),
-                       p(o_ray), p(o_conf), p(o_uv), p(o_match), p(o_order), p(o_nm), p(o_xr))
-    L_.check(lib.mlb_post_process(C.byref(a), _stream(dev)), 'mlb_post_process')
-    xyz, conf, uv = o_xyz.cpu().numpy(), o_conf.cpu().numpy(), o_uv.cpu().numpy()
-    match, order, nm, xr = o_match.cpu().numpy(), o_order.cpu().numpy(), o_nm.cpu().numpy(), o_xr.cpu().numpy()
-
+    out = post_process_device(t(np.asarray(det_off, dtype=np.int32), torch.int32), t(np.concatenate(boxes), torch.float64),
+                              t(np.concatenate(kps), torch.float32), t(np.stack(kinv), torch.float32),
+                              t(np.concatenate(dec), torch.float32), max(np.diff(det_off)),
+                              gt={k: torch.from_numpy(v).to(dev) if isinstance(v, np.ndarray) else v
+                                  for k, v in gt.items()} if gt else None,
+                              iou_min=iou_min, reorder=reorder)
+    host = {k: v.cpu().numpy() for k, v in out.items()}
     for li, i in enumerate(live):
         dic_in, bx, kp, kk, dic_gt = items[i]
-        res = results[i]
-        d0, m = det_off[li], det_off[li + 1] - det_off[li]
-        n_match = int(nm[li])
-        res['gt'] = [True] * n_match + [False] * (m - n_match)
-        dd = np.asarray(dic_in['d'], dtype=np.float64).reshape(-1)
-        bi = np.asarray(dic_in['bi'], dtype=np.float64).reshape(-1)
-        epi = np.asarray(dic_in['epi'], dtype=np.float64).reshape(-1)
-        has_yaw, has_aux = 'yaw' in dic_in, 'aux' in dic_in
-        for pos in range(m):
-            j = int(order[d0 + pos])
-            res['boxes'].append(bx[j])
-            res['confs'].append(float(conf[d0 + j]))
-            res['dds_pred'].append(float(dd[j]))
-            res['stds_ale'].append(float(bi[j]))
-            res['stds_epi'].append(float(epi[j]))
-            res['xyz_pred'].append(xyz[d0 + j].tolist())
-            res['uv_kps'].append(kp[j])
-            res['uv_centers'].append([int(uv[d0 + j, 0]), int(uv[d0 + j, 1])])
-            res['uv_shoulders'].append([int(uv[d0 + j, 2]), int(uv[d0 + j, 3])])
-            res['uv_heads'].append([int(uv[d0 + j, 4]), int(uv[d0 + j, 5])])
-            res['angles']
-            if not has_yaw:
-                continue
-            res['angles'].append(float(dic_in['yaw'][0][j]))
-            res['angles_egocentric'].append(float(dic_in['yaw'][1][j]))
-            res['aux']
-            if has_aux:
-                res['aux'].append(float(dic_in['aux'][j]))
-        for pos in range(n_match):  # net.py:242-247, in the (re)ordered match order
-            j = int(order[d0 + pos])
-            jg = int(match[d0 + j])
-            res['dds_real'].append(dic_gt['ys'][jg][3])
-            res['boxes_gt'].append(dic_gt['boxes'][jg])
-            res['xyz_real'].append(xr[d0 + j].tolist())
+        a, b = det_off[li], det_off[li + 1]
+        col = lambda v: np.asarray(v, dtype=np.float64).reshape(-1)  # noqa: E731
+        yaw = (col(dic_in['yaw'][0]), col(dic_in['yaw'][1])) if 'yaw' in dic_in else None
+        assemble_post(results[i], {k: host[k][a:b] for k in ('xyz', 'conf', 'uv', 'match', 'order', 'xyz_real')},
+                      int(host['n_match'][li]), bx, kp, col(dic_in['d']), col(dic_in['bi']), col(dic_in['epi']), yaw,
+                      col(dic_in['aux']) if 'aux' in dic_in else None, dic_gt)
     return results
+
+
+def gt_arrays(dic_gt_list):
+    """Ground truths of the images (dic_gt or None each) as the CSR arrays mlb_post_process reads: numpy gt_off [n_img + 1]
+    int32, gt_boxes [n_gt, 4] fp64, gt_d [n_gt] fp64 (dic_gt['ys'][j][3]) and max_gt; None when no image has any."""
+    gt_off, gtb, gtd = [0], [], []
+    for dic_gt in dic_gt_list:
+        g = len(dic_gt['boxes']) if dic_gt else 0
+        if g:
+            gtb.append(np.asarray(dic_gt['boxes'], dtype=np.float64).reshape(g, -1)[:, :4])
+            gtd.append(np.asarray([y[3] for y in dic_gt['ys']], dtype=np.float64))
+        gt_off.append(gt_off[-1] + g)
+    if not gtb:
+        return None
+    return {'gt_off': np.asarray(gt_off, dtype=np.int32), 'gt_boxes': np.concatenate(gtb), 'gt_d': np.concatenate(gtd),
+            'max_gt': int(np.diff(gt_off).max())}
+
+
+def post_process_device(det_off, boxes, kps, kinv, dec, max_det, gt=None, iou_min=0.3, reorder=True):
+    """`mlb_post_process` on device tensors, no host synchronisation: det_off [n_img + 1] int32 CSR, boxes [n, 5] fp64,
+    kps [n, 3, 17] fp32, kinv [n_img, 9] fp32, dec [n, 8] fp32 (d at 3, bi at 4), max_det the largest image; gt the
+    gt_arrays dictionary with its arrays as CUDA tensors, or None.  Returns CUDA tensors xyz [n, 3], conf [n], uv [n, 6],
+    match [n] (image-local gt index or -1), order [n] (image-local detection at every output position), n_match [n_img]
+    and xyz_real [n, 3]."""
+    lib = L_.lib()
+    dev = boxes.device
+    n, n_img = boxes.shape[0], det_off.numel() - 1
+    out = {'xyz': torch.empty((n, 3), dtype=torch.float32, device=dev),
+           'ray': torch.empty((n, 4), dtype=torch.float32, device=dev),
+           'conf': torch.empty((n,), dtype=torch.float64, device=dev),
+           'uv': torch.empty((n, 6), dtype=torch.int32, device=dev),
+           'match': torch.empty((n,), dtype=torch.int32, device=dev),
+           'order': torch.empty((n,), dtype=torch.int32, device=dev),
+           'n_match': torch.empty((n_img,), dtype=torch.int32, device=dev),
+           'xyz_real': torch.zeros((n, 3), dtype=torch.float32, device=dev)}
+    p = lambda x: x.data_ptr() if x is not None else None  # noqa: E731
+    g = gt or {}
+    a = L_.MlbPostArgs(n_img, int(max_det), int(g.get('max_gt', 0)), int(bool(reorder)), float(iou_min), p(det_off),
+                       p(g.get('gt_off')), p(boxes), p(kps), p(kinv), p(dec), p(g.get('gt_boxes')), p(g.get('gt_d')),
+                       p(out['xyz']), p(out['ray']), p(out['conf']), p(out['uv']), p(out['match']), p(out['order']),
+                       p(out['n_match']), p(out['xyz_real']))
+    L_.check(lib.mlb_post_process(C.byref(a), _stream(dev)), 'mlb_post_process')
+    del out['ray']
+    return out
+
+
+def assemble_post(res, dev, n_match, boxes, keypoints, dd, bi, epi, yaw, aux, dic_gt):
+    """Fill `res` (a defaultdict(list)) for one image of m >= 1 detections with the keys, key order and values of
+    net.py:164-248.  dev: that image's rows of post_process_device's outputs as numpy arrays (image-local); boxes /
+    keypoints the caller's lists (their elements are placed in the result as they are); dd, bi, epi fp64 columns by
+    detection; yaw (angles, egocentric angles) or None; aux or None."""
+    o = dev['order'].astype(np.int64)
+    m = len(o)
+    res['gt'] = [True] * n_match + [False] * (m - n_match)
+    res['boxes'] = [boxes[j] for j in o]
+    res['confs'] = dev['conf'][o].tolist()
+    res['dds_pred'] = dd[o].tolist()
+    res['stds_ale'] = bi[o].tolist()
+    res['stds_epi'] = epi[o].tolist()
+    res['xyz_pred'] = dev['xyz'][o].tolist()
+    res['uv_kps'] = [keypoints[j] for j in o]
+    uv = dev['uv'][o]
+    res['uv_centers'], res['uv_shoulders'], res['uv_heads'] = uv[:, 0:2].tolist(), uv[:, 2:4].tolist(), uv[:, 4:6].tolist()
+    res['angles']  # the reference's defaultdict access creates these keys even when the value is missing
+    if yaw is not None:
+        res['angles'] = yaw[0][o].tolist()
+        res['angles_egocentric'] = yaw[1][o].tolist()
+        res['aux']
+        if aux is not None:
+            res['aux'] = aux[o].tolist()
+    if n_match:  # net.py:242-247, in the (re)ordered match order
+        om = o[:n_match]
+        jg = dev['match'][om].tolist()
+        res['dds_real'] = [dic_gt['ys'][k][3] for k in jg]
+        res['boxes_gt'] = [dic_gt['boxes'][k] for k in jg]
+        res['xyz_real'] = dev['xyz_real'][om].tolist()
+    return res
 
 
 def kitti_rows_device(boxes, raw, dec, epi=None, net='monoloco_pp'):

@@ -4,12 +4,15 @@ preprocess_monoloco / preprocess_monstereo / extract_outputs / unnormalize_bi / 
 reference's names, argument meaning and error behaviour (asserts) but run on the GPU through
 libmonoloco_b200.so; the host-side list munging (pifpaf json -> lists, calibration yaml) is plain Python.
 """
+import ctypes as C
 import json
+import math
 import os
 
 import numpy as np
 import torch
 
+from .. import _lib as L_
 from ..engine import preprocess_device
 
 Sx, Sy = 7.2, 5.4  # nuScenes sensor size in mm (process.py:21-22)
@@ -159,3 +162,93 @@ def preprocess_pifpaf(annotations, im_size=None, enlarge_boxes=True, min_conf=0.
             boxes.append(box)
             keypoints.append(kps)
     return boxes, keypoints
+
+
+# ------------------------------------------------------------------------------------------------ many images on the device
+PIFPAF_FIELDS = (('kps', np.float64), ('bbox', np.float64), ('score', np.float64), ('im_size', np.float64),
+                 ('ann_off', np.int32), ('has_score', np.uint8), ('has_size', np.uint8))
+
+
+def check_pifpaf_options(enlarge_boxes, min_conf):
+    """(enlarge, min_conf) as mlb_preprocess_pifpaf takes them; ValueError for a non-bool enlarge_boxes or a min_conf
+    that is not a finite number."""
+    if not isinstance(enlarge_boxes, (bool, np.bool_)):
+        raise ValueError("enlarge_boxes must be True or False")
+    try:
+        mc = float(min_conf)
+    except (TypeError, ValueError):
+        raise ValueError("min_conf must be a finite number") from None
+    if not math.isfinite(mc):
+        raise ValueError("min_conf must be a finite number")
+    return (1 if enlarge_boxes else 2), mc
+
+
+def pack_pifpaf(annotations_list, im_size_list):
+    """pifpaf annotations of many images -> the numpy arrays mlb_preprocess_pifpaf reads (PIFPAF_FIELDS): ann_off
+    [n_img + 1] CSR, kps [n, 51] and bbox [n, 4] fp64, score [n] with has_score [n] (the 'score' key), im_size [n_img, 2]
+    with has_size [n_img] (None: no clamping).  The annotation dictionaries are only read."""
+    n_img = len(annotations_list)
+    if len(im_size_list) != n_img:
+        raise ValueError("one image size (or None) per image: %d for %d images" % (len(im_size_list), n_img))
+    counts = [len(a) for a in annotations_list]
+    anns = [d for a in annotations_list for d in a]
+    n = len(anns)
+    try:
+        kps = np.asarray([d['keypoints'] for d in anns], dtype=np.float64).reshape(n, -1) if n else np.zeros((0, 51))
+        bbox = np.asarray([d['bbox'] for d in anns], dtype=np.float64).reshape(n, -1) if n else np.zeros((0, 4))
+    except (KeyError, TypeError, ValueError) as e:
+        raise ValueError("every annotation needs 'keypoints' (51 numbers) and 'bbox' (4 numbers): %s" % e) from None
+    if kps.shape[1] != 51 or bbox.shape[1] != 4:
+        raise ValueError("every annotation needs 'keypoints' (51 numbers) and 'bbox' (4 numbers)")
+    has_score = np.fromiter(('score' in d for d in anns), dtype=np.uint8, count=n)
+    score = np.asarray([d['score'] if 'score' in d else 0.0 for d in anns], dtype=np.float64).reshape(n)
+    im_size = np.zeros((n_img, 2), dtype=np.float64)
+    has_size = np.zeros(n_img, dtype=np.uint8)
+    for i, sz in enumerate(im_size_list):
+        if sz is not None:
+            if len(sz) != 2:
+                raise ValueError("image size %d: (width, height) or None" % i)
+            im_size[i] = (float(sz[0]), float(sz[1]))
+            has_size[i] = 1
+    ann_off = np.zeros(n_img + 1, dtype=np.int64)
+    np.cumsum(counts, out=ann_off[1:])
+    if ann_off[-1] > np.iinfo(np.int32).max:
+        raise ValueError("more than 2^31 - 1 annotations")
+    return {'kps': kps, 'bbox': bbox, 'score': score, 'im_size': im_size, 'ann_off': ann_off.astype(np.int32),
+            'has_score': has_score, 'has_size': has_size}
+
+
+def pifpaf_layout(packs):
+    """Byte layout of several packs (pack_pifpaf) in one buffer: list of {field: (byte offset, shape, numpy dtype)} per
+    pack, and the total size.  Every field starts on an 8-byte boundary."""
+    out, pos = [], 0
+    for p in packs:
+        lay = {}
+        for name, dt in PIFPAF_FIELDS:
+            a = p[name]
+            lay[name] = (pos, a.shape, np.dtype(dt))
+            pos += -(-a.size * np.dtype(dt).itemsize // 8) * 8
+        out.append(lay)
+    return out, max(pos, 8)
+
+
+def preprocess_pifpaf_device(arrays, n_img, n_ann, enlarge, min_conf):
+    """mlb_preprocess_pifpaf on device tensors (`arrays`: the PIFPAF_FIELDS of one pack as CUDA tensors), no host
+    synchronisation.  Returns CUDA tensors boxes [n_ann, 5] fp64, kps [n_ann, 3, 17] fp64, kps32 fp32, src [n_ann],
+    kept_off [n_img + 1] and error [1]; rows beyond kept_off[-1] are unused."""
+    dev = arrays['kps'].device
+    e = lambda shape, dt: torch.empty(shape, dtype=dt, device=dev)  # noqa: E731
+    out = {'boxes': e((n_ann, 5), torch.float64), 'kps': e((n_ann, 3, 17), torch.float64),
+           'kps32': e((n_ann, 3, 17), torch.float32), 'src': e((n_ann,), torch.int32),
+           'kept_off': e((n_img + 1,), torch.int32), 'error': e((1,), torch.int32)}
+    scratch = e((n_img + 1,), torch.int64)
+    p = lambda t: t.data_ptr() if t.numel() else None  # noqa: E731
+    a = L_.MlbPifpafArgs()
+    a.n_img, a.n_ann, a.enlarge, a.min_conf = n_img, n_ann, enlarge, min_conf
+    a.ann_off, a.kps, a.bbox, a.score = p(arrays['ann_off']), p(arrays['kps']), p(arrays['bbox']), p(arrays['score'])
+    a.has_score, a.im_size, a.has_size = p(arrays['has_score']), p(arrays['im_size']), p(arrays['has_size'])
+    a.out_boxes, a.out_kps, a.out_kps32, a.out_src = p(out['boxes']), p(out['kps']), p(out['kps32']), p(out['src'])
+    a.kept_off, a.error, a.scratch = p(out['kept_off']), p(out['error']), p(scratch)
+    L_.check(L_.lib().mlb_preprocess_pifpaf(C.byref(a), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+             'mlb_preprocess_pifpaf')
+    return out
